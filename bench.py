@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- pseudo-label images/s of the IRN hot path on B200 (BASELINE.json metric).
+"""bench.py -- pseudo-label images/s of the IRN hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config 2|3|4|5] [--batch B] [--impl reference]
 
@@ -34,7 +34,7 @@ H = W = 512
 SCALES = (1.0, 0.5, 1.5, 2.0)
 GFLOP_CAM, GFLOP_IRN = 974.04, 149.61       # SURVEY.md section 8(d): 4-scale CAM, EdgeDisplacement, per image
 N_TRAIN_AUG = 10582
-CONV_MODES = {0: "SIMT fp32", 1: "tcgen05 3xTF32", 2: "tcgen05 f16x3 (fp16 hi/lo split operands, fp32 accumulate)"}
+CONV_MODES = {0: "SIMT fp32", 1: "wgmma 3xTF32", 2: "wgmma f16x3 (fp16 hi/lo split operands, fp32 accumulate)"}
 
 
 def parse():
@@ -48,10 +48,12 @@ def parse():
     ap.add_argument("--parity-images", type=int, default=8)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
-    ap.add_argument("--conv-mode", type=int, default=-1, help="0 SIMT fp32, 1 tcgen05 3xTF32, 2 tcgen05 f16x3; -1 = library default")
+    ap.add_argument("--conv-mode", type=int, default=-1, help="0 SIMT fp32, 1 wgmma 3xTF32, 2 wgmma f16x3; -1 = library default")
     ap.add_argument("--list-limit", type=int, default=0, help="--config 4: ids in the list (default 10,582 * N / 8)")
     ap.add_argument("--step-batch", type=int, default=64, help="--config 4: --step_batch of the step entry points")
     ap.add_argument("--num-workers", type=int, default=-1, help="--config 4: DataLoader workers per GPU")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the timed path returned in its last step as DIR/<name>.npy (float32, <= 64 MB in all)")
     a = ap.parse_args()
     if a.batch <= 0:
         a.batch = 32 if a.config == 5 else 64
@@ -75,13 +77,13 @@ def config(a, n_gpus):
            "inputs": "decoded uint8 images [batch,512,512,3]; the 4-scale bicubic / normalise / flip pyramids (C1) are built on the device "
                      "inside the timed region",
            "l2": "every step writes and re-reads %.1f GB of fp32 pyramids plus the activations between two reads of the inputs: "
-                 "far beyond the 126 MB L2, nothing survives from one step to the next" % (batch * 47.2e6 / 1e9),
+                 "far beyond the 50 MB L2, nothing survives from one step to the next" % (batch * 47.2e6 / 1e9),
            "weights": "seeded synthetic checkpoints in the reference's state_dict format (irn_b200/synth.py)"}
     return cfg
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -114,7 +116,7 @@ class ClockSampler(threading.Thread):
 
 
 def cpu_threads():
-    # measured on the B200 host (profiles/r01_cpu_threads_probe.txt): 128 torch threads are 50x slower than 16-32
+    # torch CPU ops on many-core hosts slow down with more than a few dozen threads (tests/probe_cpu_threads.py measures it)
     return min(os.cpu_count(), int(os.environ.get("IRN_CPU_THREADS", "32")))
 
 
@@ -207,7 +209,7 @@ def _claim_stdout():
 
 # ----------------------------------------------------------------------------------------------- torch-eager context arm
 def eager_baseline(dev, batch_images):
-    """The 'existing Blackwell path' for the convolution part (BASELINE.md section 3): the oracle's functional restatement of
+    """The existing GPU path for the convolution part (BASELINE.md section 3): the oracle's functional restatement of
     the reference networks run by torch eager on this GPU (cuDNN / ATen), CAM forward at the four scales + IRNet forward on
     `batch_images` image pairs -- with cuDNN's TF32 convolutions (torch's default; misses the 1e-4 contract by ~20x, SURVEY.md
     H1) and with allow_tf32=False (IEEE fp32, the accuracy-equivalent arm).  Context only: it is not the reference arm."""
@@ -394,6 +396,16 @@ def run_config4(a, rank, world, local, dev, out_stream):
                     "api": "step.make_cam._work + step.make_sem_seg_labels._work (reference entry points), files in / files out"},
             "gpu_launches": launches, "clocks": clocks, "conv_mode": conv_mode_name(L, cam, dev)}
     if rank == 0:
+        if a.dump_outputs:
+            # what the last pass wrote for the first ids of this rank's shard: stride-4 CAMs (.npy) and label maps (.png)
+            from PIL import Image
+            last = "run%d" % (a.steps - 1)
+            names = sorted(n[:-4] for n in os.listdir(os.path.join(root, "out_%s_sem" % last)))[:DUMP_IMAGES]
+            cams = [np.load(os.path.join(root, "out_%s_cam" % last, n + ".npy"), allow_pickle=True).item() for n in names]
+            dump_outputs(a.dump_outputs, {
+                "cam_keys": np.concatenate([np.asarray(c["keys"]) for c in cams]), "cam_counts": [len(c["keys"]) for c in cams],
+                "cams": np.concatenate([np.asarray(c["cam"]) for c in cams]),
+                "labels": np.stack([np.asarray(Image.open(os.path.join(root, "out_%s_sem" % last, n + ".png"))) for n in names])})
         out_stream.write(json.dumps(line) + "\n")
         out_stream.flush()
         shutil.rmtree(root, ignore_errors=True)
@@ -404,6 +416,46 @@ def conv_mode_name(L, cam, dev):
         return CONV_MODES.get(int(L.irn_net_get_conv_mode(cam._get_plan(dev).handle)), "?")
     except Exception:
         return "?"
+
+
+# ----------------------------------------------------------------------------------------------- --dump-outputs
+DUMP_IMAGES = 16      # per-pixel full-resolution maps are written for the first images of the batch only: 64 MB would hold 64
+
+
+def dump_outputs(d, arrays):
+    """arrays: name -> array-like; written as float32 .npy files (same names, same shapes from run to run)."""
+    os.makedirs(d, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        a = a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+        a = np.ascontiguousarray(a, dtype=np.float32)
+        total += a.nbytes
+        np.save(os.path.join(d, name + ".npy"), a)
+    assert total <= 64 << 20, "dumped outputs exceed 64 MB (%d bytes)" % total
+
+
+def step_arrays(config, out):
+    """The arrays a caller of the timed path receives from one step, as float32."""
+    import torch
+    keys = [np.asarray(k) for k in out["keys"]]
+    a = {"cam_keys": np.concatenate(keys) if keys else np.zeros(0), "cam_counts": np.array([len(k) for k in keys])}
+    if config in (2, 3):
+        a["cams"] = torch.cat(list(out["cams"]), 0)                       # stride-4 CAMs of every image, [sum K_i, h4, w4]
+    if config == 3:
+        a["labels"] = out["labels"][:DUMP_IMAGES]                          # sem-seg label maps, [16, H, W]
+        a["edge"] = out["edge"]
+        a["dp"] = out["dp"]
+    if config == 2:
+        n = int(sum(len(k) for k in keys[:DUMP_IMAGES]))
+        a["high_res"] = torch.cat(list(out["high_res"]), 0)[:n]           # full-resolution CAMs of the first 16 images
+    if config == 5:
+        dets = out["detections"]
+        a["det_counts"] = np.array([0 if d is None else len(d["score"]) for d in dets])
+        a["det_scores"] = np.concatenate([np.asarray(d["score"], np.float32) for d in dets if d is not None] or [np.zeros(0)])
+        a["det_classes"] = np.concatenate([np.asarray(d["class"]) for d in dets if d is not None] or [np.zeros(0)])
+        masks = [np.asarray(d["mask"]) for d in dets[:DUMP_IMAGES] if d is not None]
+        a["det_masks"] = np.concatenate(masks) if masks else np.zeros((0, H, W))   # masks of the first 16 images' detections
+    return a
 
 
 # ----------------------------------------------------------------------------------------------- main
@@ -570,6 +622,8 @@ def main():
     L.irn_rw_set_timing(1)
     launches0 = L.irn_total_launch_count()
     ms_dev, wall_dev, out, per_rank_ms = timed(a.steps, False)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, step_arrays(a.config, out))
     launches = int(L.irn_total_launch_count() - launches0)
     import ctypes
     step_ms, n_it = ctypes.c_float(), ctypes.c_int()
@@ -611,7 +665,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))     # fallback: H100 SXM data sheet
     roofline = None
     if have_rw and a.config == 3:
         counts = [len(k) for k in out["keys"]]
@@ -619,45 +673,33 @@ def main():
         n_img, totc, N = len(last), sum(last), (H // 4) * (W // 4)
         # SURVEY.md section 8(d) B_rw per walk step with e = 8 (fp64 state): N * [4*34 (A^beta) + 4 (1/s)] per image + 2*8*N per channel
         alg_step = N * (n_img * (4 * 34 + 4) + 2 * 8 * totc)
-        src = "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s"
+        src = "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet 3350 GB/s (not measured)"
         if L.irn_rw_last_was_fused():
             # the whole walk is ONE launch: algorithmic bytes = n_iter x the per-step figure (SURVEY.md 8(d) B_rw; DESIGN.md 4)
             launch_ms = step_ms.value * n_it.value
             alg = alg_step * n_it.value
-            traffic = None
-            try:
-                t = json.load(open(os.path.join(ROOT, "profiles", "rw_fused_traffic.json")))
-                traffic = int(t["dram_bytes_per_item"] * totc)
-            except Exception:
-                pass
             ach = alg / (launch_ms * 1e-3) / 1e9
             wf_per_warp_step = (34 * 2 - 16) * 4 + 108 * 2      # weight LDS.32 (16 planes' forward taps come from registers) + state LDS.64 x 2 wavefronts
             clusters = max(1, int(L.irn_rw_last_was_fused()))
             per = -(-totc // clusters)                         # items walked by the busiest cluster
             smem_cycles = wf_per_warp_step * 8 * per * n_it.value   # 8 warps per CTA, one 128-byte wavefront per cycle per SM
             roofline = {"kernel": "rw_fused_kernel", "bound": "hbm", "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": ach / hbm,
-                        "traffic": traffic, "peak_source": src, "launch_us": 1e3 * launch_ms, "steps_per_launch": n_it.value,
+                        "peak_source": src, "launch_us": 1e3 * launch_ms, "steps_per_launch": n_it.value,
                         "images_per_launch": n_img, "channels_per_launch": totc, "algorithmic_bytes_per_launch": alg,
                         "algorithmic_bytes_formula": "256 steps x N=16384 x [images x (4*34 + 4) + channels x 2*8] (SURVEY.md 8(d), fp64 state)",
-                        "note": "weights stay resident in shared memory for all steps of a launch, so DRAM traffic (`traffic`) is a small "
-                                "fraction of the algorithmic bytes and frac may exceed 1; the kernel's real ceiling is shared-memory bandwidth, which scales "
-                                "with the SM clock: the launch is timed INSIDE the step, at the clock the power cap leaves the conv kernels "
-                                "(`clocks.sm_mhz`): 0.80 at ~1830 MHz (round 1's lighter conv path), ~0.70 at ~1570 MHz; it occupies 7 clusters x 16 "
-                                "CTAs = 112 of 148 SMs (one 16-CTA cluster per GPC that has 16 free SMs)",
+                        "note": "weights stay resident in shared memory for all steps of a launch, so DRAM traffic is a small fraction of the "
+                                "algorithmic bytes and frac may exceed 1; the kernel's real ceiling is shared-memory bandwidth, which scales with the SM "
+                                "clock: the launch is timed INSIDE the step, at the clock the power cap leaves the conv kernels (`clocks.sm_mhz`); "
+                                "`clusters` thread-block clusters of up to 16 CTAs are co-resident",
                         "clusters": clusters, "smem_wavefront_frac": smem_cycles / (launch_ms * 1e-3 * clocks_mhz(clocks) * 1e6)}
         else:
-            traffic = None
-            try:
-                traffic = json.load(open(os.path.join(ROOT, "profiles", "rw_step_traffic.json")))["dram_bytes_per_launch"]
-            except Exception:
-                pass
             ach = alg_step / (step_ms.value * 1e-3) / 1e9
             roofline = {"kernel": "rw_step_tma_kernel", "bound": "hbm", "achieved": ach, "peak": hbm, "unit": "GB/s", "frac": ach / hbm,
-                        "traffic": traffic, "peak_source": src, "launch_us": 1e3 * step_ms.value, "images_per_launch": n_img,
+                        "peak_source": src, "launch_us": 1e3 * step_ms.value, "images_per_launch": n_img,
                         "channels_per_launch": totc, "algorithmic_bytes_per_launch": alg_step}
     mode = int(L.irn_net_get_conv_mode(cam._get_plan(dev).handle))
     mode_irn = int(L.irn_net_get_conv_mode(irn._get_plan(dev).handle))
-    bf16_peak = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    bf16_peak = float(peaks.get("bf16_tflops_sustained", 989.0))     # fallback: H100 SXM data sheet, dense
     tf32_peak = bf16_peak / 2.0
     roofline_conv = None
     if conv_ms:
@@ -667,10 +709,11 @@ def main():
         cam_peak = bf16_peak if mode == 2 else tf32_peak
         irn_peak = bf16_peak if mode_irn == 2 else tf32_peak
         t_issued = 3 * B * GFLOP_CAM / cam_peak + (3 * B * GFLOP_IRN / irn_peak if a.config == 3 else 0.0)      # ms
-        roofline_conv = {"bound": "tensor", "kernel": "conv_tc_* (tcgen05 implicit-GEMM convolutions)", "achieved": ach_tf, "unit": "TFLOP/s",
+        roofline_conv = {"bound": "tensor", "kernel": "conv_wg_kernel (wgmma implicit-GEMM convolutions)", "achieved": ach_tf, "unit": "TFLOP/s",
                          "peak": cam_peak, "frac": ach_tf / cam_peak, "frac_issued": t_issued / conv_ms,
                          "conv_path_ms_per_step": conv_ms, "share_of_step": conv_ms / (ms_dev / a.steps),
-                         "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained%s" % (" (kind::f16 MMAs run at the bf16 rate)" if mode == 2 else " / 2 (tf32 runs at half the bf16 rate)"),
+                         "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "H100 SXM data sheet 989 TFLOP/s (not measured)") +
+                                        (" (f16 MMAs run at the bf16 rate)" if mode == 2 else " / 2 (tf32 runs at half the bf16 rate)"),
                          "note": "achieved = algorithmic conv FLOPs (974.04 CAM + 149.61 IRNet GFLOP/image) / CUDA-event time of the CAM x4-scale and "
                                  "IRNet forwards of one batch (re-run after the timed region; includes their ~4% of pooling / GroupNorm glue kernels); "
                                  "frac = achieved / peak of the MMA kind the CAM trunk uses; frac_issued = tensor time of the issued MMAs (3 per "

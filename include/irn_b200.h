@@ -1,5 +1,5 @@
 /*
- * irn_b200.h -- C ABI of libirn_b200.so: the B200 (sm_100a) implementation of the IRN
+ * irn_b200.h -- C ABI of libirn_b200.so: the H100 (sm_90a) implementation of the IRN
  * pseudo-label hot path (jiwoon-ahn/irn).
  *
  * The reference has no FFI of its own (pure Python on torch); its seams are Python names
@@ -146,10 +146,9 @@ typedef struct irn_net irn_net;
 int irn_cam_net_create(const float* params, size_t n_floats, irn_net** out);
 int irn_irn_net_create(const float* params, size_t n_floats, irn_net** out);
 void irn_net_destroy(irn_net* net);
-/* Convolution arithmetic: 2 (default) = tcgen05 tensor cores, f16x3 split (fp16 hi/lo operand parts, fp32 accumulation in
- * separated TMEM accumulators: fp32-grade, ~22 bits per operand) for every conv with Cin % 64 == 0 and Cout % 64 == 0,
- * 3xTF32 for the stem, SIMT fp32 for the rest; 1 = 3xTF32 split (round-1 kernels, Cin % 32 == 0) instead; 0 = SIMT IEEE
- * fp32 everywhere (the on-device cross-check). */
+/* Convolution arithmetic: 2 (default) = wgmma tensor cores, f16x3 split (fp16 hi/lo operand parts, per-k-block fp32 partial
+ * sums added in IEEE fp32: fp32-grade, ~22 bits per operand) for every conv with Cin % 64 == 0 and Cout % 64 == 0 and the stem,
+ * SIMT fp32 for the rest; 1 = 3xTF32 split (Cin % 32 == 0) instead; 0 = SIMT IEEE fp32 everywhere (the on-device cross-check). */
 int irn_net_set_conv_mode(irn_net* net, int mode);
 int irn_net_get_conv_mode(const irn_net* net);
 

@@ -36,7 +36,7 @@ class CAM(CamParams):
         self._conv_mode = None      # None = the library's default for this network
 
     def set_conv_mode(self, mode):
-        """Convolution arithmetic of the native plan: 0 SIMT fp32, 1 tcgen05 3xTF32, 2 tcgen05 bf16x3 (irn_net_set_conv_mode)."""
+        """Convolution arithmetic of the native plan: 0 SIMT fp32, 1 wgmma 3xTF32, 2 wgmma f16x3 (irn_net_set_conv_mode)."""
         self._conv_mode = None if mode is None else int(mode)
         if self._plan is not None and self._conv_mode is not None:
             _lib.check(_lib.lib().irn_net_set_conv_mode(self._plan.handle, self._conv_mode), "irn_net_set_conv_mode")

@@ -1,5 +1,5 @@
 // SIMT fp32 implicit-GEMM convolution (NHWC) and the small glue kernels of the network path.
-// This is the exact-fp32 path: every conv the tcgen05 kernel (conv_tc.cu) does not cover runs
+// This is the exact-fp32 path: every conv the wgmma kernel (conv_wgmma.cuh) does not cover runs
 // here, and it is the on-device cross-check for the tensor-core path.
 //
 // Reference semantics restated (SURVEY.md App. E): cross-correlation, zero padding, no bias;

@@ -16,8 +16,7 @@
 
 #include "common.h"
 #include "conv_simt.cuh"
-#include "conv_tc.cuh"
-#include "conv_f16.cuh"
+#include "conv_wgmma.cuh"
 
 namespace irn {
 
@@ -30,8 +29,7 @@ struct Conv {
     float* w_lo = nullptr;
     int bn = 0;              // N tile (64 or 128); 0 = not eligible
     CUtensorMap map_bhi, map_blo;        // box {32, bn}
-    CUtensorMap map_bhi64, map_blo64;    // box {32, 64} (short-K configuration)
-    // f16x3 path (conv_f16.cuh): weights [cout][k*k*cin], pre-scaled per output channel by a power of two and split into fp16
+    // f16x3 path (conv_wgmma.cuh): weights [cout][k*k*cin], pre-scaled per output channel by a power of two and split into fp16
     // hi / lo parts, boxes {64 k, 64 | 128 rows}; oscale[cout] = the inverse scale applied in the epilogue
     uint16_t* wb_hi = nullptr;
     uint16_t* wb_lo = nullptr;
@@ -62,7 +60,7 @@ struct Block {
 
 struct irn_net {
     int kind = 0;   // 0 = CAM, 1 = IRN (EdgeDisplacement)
-    int conv_mode = 2;   // 0 = SIMT exact-fp32 convolutions only, 1 = tcgen05 3xTF32 where eligible, 2 = tcgen05 f16x3 (default; 3xTF32 / SIMT for the layers it cannot take)
+    int conv_mode = 2;   // 0 = SIMT exact-fp32 convolutions only, 1 = wgmma 3xTF32 where eligible, 2 = wgmma f16x3 (default; 3xTF32 / SIMT for the layers it cannot take)
     irn::Conv stem;
     irn::Conv stem_f16;            // the stem repacked for the f16x3 kernel (K = 256 over the NHWC4 halo layout)
     std::vector<irn::Block> blocks[4];
@@ -168,9 +166,6 @@ static int read_conv(irn_net* net, Reader& rd, Conv& c, int cin, int cout, int k
         const uint32_t box[2] = {(uint32_t)kTcBK, (uint32_t)c.bn};
         if ((rc = make_tensor_map(&c.map_bhi, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c.w_hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
         if ((rc = make_tensor_map(&c.map_blo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c.w_lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-        const uint32_t box64[2] = {(uint32_t)kTcBK, 64};
-        if ((rc = make_tensor_map(&c.map_bhi64, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c.w_hi, dims, strides, box64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-        if ((rc = make_tensor_map(&c.map_blo64, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c.w_lo, dims, strides, box64, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
     }
     return kOk;
 }
@@ -318,191 +313,79 @@ static int read_head(irn_net* net, Reader& rd, Head& h, int cin, int cout, int g
 // ------------------------------------------------------------------ launch helpers
 static inline int conv_out(int n, int k, int s, int p) { return (n + 2 * p - k) / s + 1; }
 
-template <int BN, int STAGES, int NACC>
-static int launch_tc(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out, bool relu,
-                     cudaStream_t st) {
+template <bool F16, int BN>
+static int launch_wg(const TcMaps& maps, const TcArgs& a, cudaStream_t st) {
+    using Cfg = WgCfg<F16, BN>;
     static DeviceOnce once;
     const int ds = once.slot();
     if (once.need(ds)) {
-        IRN_CUDA(cudaFuncSetAttribute((conv_tc_kernel<BN, STAGES, NACC>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(BN, STAGES)));
+        IRN_CUDA(cudaFuncSetAttribute((conv_wg_kernel<F16, BN>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
         once.done[ds] = true;
     }
-    TcMaps maps;
-    maps.b_hi = BN == 64 && c.bn == 128 ? c.map_bhi64 : c.map_bhi;
-    maps.b_lo = BN == 64 && c.bn == 128 ? c.map_blo64 : c.map_blo;
-    const uint64_t dims[4] = {(uint64_t)c.cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
-    const uint64_t strides[3] = {(uint64_t)c.cin * 4, (uint64_t)W * c.cin * 4, (uint64_t)H * W * c.cin * 4};
-    const uint32_t box[4] = {(uint32_t)kTcBK, (uint32_t)(kTcTW * c.stride), (uint32_t)(kTcTH * c.stride), 1};
-    const uint32_t estr[4] = {1, (uint32_t)c.stride, (uint32_t)c.stride, 1};
-    int rc = make_tensor_map(&maps.a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, in, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
-    if (rc) return rc;
+    const long long grid = (long long)a.tiles_x * a.tiles_y * a.B * (a.Cout / BN);
+    conv_wg_kernel<F16, BN><<<(unsigned)grid, kWgThreads, Cfg::kSmem, st>>>(maps, a);
+    IRN_LAUNCH_CHECK(F16 ? "conv_wg_kernel<f16x3>" : "conv_wg_kernel<3xtf32>");
+    return kOk;
+}
+
+static TcArgs conv_args(const Conv& c, int B, int Ho, int Wo, const float* residual, float* out, bool relu) {
     TcArgs a;
     a.bias = c.bias; a.residual = residual; a.out = out;
+    a.oscale = c.oscale;
     a.B = B; a.Ho = Ho; a.Wo = Wo; a.Cout = c.cout; a.Cin = c.cin; a.ksize = c.k; a.stride = c.stride; a.pad = c.pad;
     a.relu = relu ? 1 : 0;
     a.tiles_x = (Wo + kTcTW - 1) / kTcTW;
     a.tiles_y = (Ho + kTcTH - 1) / kTcTH;
-    a.mode = 0;
-    dim3 grid((unsigned)(a.tiles_x * a.tiles_y * B * (c.cout / BN)));
-    conv_tc_kernel<BN, STAGES, NACC><<<grid, kTcThreads, tc_smem_bytes(BN, STAGES), st>>>(maps, a);
-    IRN_LAUNCH_CHECK("conv_tc_kernel");
-    return kOk;
+    return a;
 }
 
-// Tensor-core stem: x4 = zero-haloed NHWC4 input [B, Hin+6, Win+8, 4]; out NHWC [B,Ho,Wo,64] with bias + ReLU.
-// A-from-TMEM persistent kernel for the 64-channel layers (IRN_TC_PERSIST_TS=0 selects the shared-memory-operand one for A/B runs)
-static bool persist_ts_enabled() {
-    static const int v = getenv("IRN_TC_PERSIST_TS") ? atoi(getenv("IRN_TC_PERSIST_TS")) : 1;
-    return v != 0;
-}
-static int persist_ts_attr() {
-    static DeviceOnce once;
-    const int ds = once.slot();
-    if (once.need(ds)) {
-        IRN_CUDA(cudaFuncSetAttribute(conv_tc_persist_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPtsSmem));
-        once.done[ds] = true;
-    }
-    return kOk;
+// NHWC fp32 [B,H,W,cin] read as boxes {32 ch, 16 px, 8 rows, 1 image} of output pixels: element strides give stride-s sampling
+static int act_map(CUtensorMap* m, const float* in, int B, int H, int W, int cin, int stride) {
+    const uint64_t dims[4] = {(uint64_t)cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
+    const uint64_t strides[3] = {(uint64_t)cin * 4, (uint64_t)W * cin * 4, (uint64_t)H * W * cin * 4};
+    const uint32_t box[4] = {32u, (uint32_t)(kTcTW * stride), (uint32_t)(kTcTH * stride), 1};
+    const uint32_t estr[4] = {1, (uint32_t)stride, (uint32_t)stride, 1};
+    return make_tensor_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, in, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
 }
 
-static int launch_tc_stem(const Conv& c, const float* x4, int B, int Hin, int Win, float* out, cudaStream_t st) {
-    static DeviceOnce once;
-    const int ds = once.slot();
-    if (once.need(ds)) {
-        IRN_CUDA(cudaFuncSetAttribute(conv_tc_persist_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcPersistCfg<64>::kSmem));
-        int dev = 0;
-        IRN_CUDA(cudaGetDevice(&dev));
-        IRN_CUDA(cudaDeviceGetAttribute(&once.n_sm[ds], cudaDevAttrMultiProcessorCount, dev));
-        once.done[ds] = true;
-    }
-    const int n_sm = once.n_sm[ds];
+// Stem input x4 = zero-haloed NHWC4 [B, Hin+6, Win+8, 4]: dim0 = the 32 contiguous floats (8 px x 4 ch) of one filter-row window,
+// dim1 = output column (windows overlap: stride 2 px = 32 B), dim2 = padded input row, dim3 = image
+static int stem_map(CUtensorMap* m, const float* x4, int B, int Hin, int Win) {
     const int Hp = Hin + 6, Wp = Win + 8;
-    const int Ho = conv_out(Hin, 7, 2, 3), Wo = conv_out(Win, 7, 2, 3);
-    TcMaps maps;
-    maps.b_hi = c.map_bhi;
-    maps.b_lo = c.map_blo;
-    // dim0: the 32 contiguous floats (8 px x 4 ch) of one filter-row window; dim1: output column (windows overlap: stride 2 px = 32 B);
-    // dim2: padded input row; dim3: image
+    const int Wo = conv_out(Win, 7, 2, 3);
     const uint64_t dims[4] = {32, (uint64_t)Wo, (uint64_t)Hp, (uint64_t)B};
     const uint64_t strides[3] = {32, (uint64_t)Wp * 16, (uint64_t)Hp * Wp * 16};
     const uint32_t box[4] = {32, (uint32_t)kTcTW, (uint32_t)(kTcTH * 2), 1};
     const uint32_t estr[4] = {1, 1, 2, 1};
-    int rc = make_tensor_map(&maps.a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
-    if (rc) return rc;
-    TcArgs a;
-    a.bias = c.bias; a.residual = nullptr; a.out = out;
-    a.B = B; a.Ho = Ho; a.Wo = Wo; a.Cout = 64; a.Cin = 32; a.ksize = 7; a.stride = 2; a.pad = 3; a.relu = 1;
-    a.tiles_x = (Wo + kTcTW - 1) / kTcTW;
-    a.tiles_y = (Ho + kTcTH - 1) / kTcTH;
-    a.mode = 1;
-    const long long total = (long long)a.tiles_x * a.tiles_y * B;
-    if (persist_ts_enabled()) {
-        int rc2 = persist_ts_attr();
-        if (rc2) return rc2;
-        conv_tc_persist_ts_kernel<<<(unsigned)(total < n_sm ? total : n_sm), kTcPersistThreads, kPtsSmem, st>>>(maps, a);
-        IRN_LAUNCH_CHECK("conv_tc_persist_ts_kernel(stem)");
-        return kOk;
-    }
-    conv_tc_persist_kernel<64><<<(unsigned)(total < n_sm ? total : n_sm), kTcPersistThreads, TcPersistCfg<64>::kSmem, st>>>(maps, a);
-    IRN_LAUNCH_CHECK("conv_tc_persist_kernel(stem)");
-    return kOk;
+    return make_tensor_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
 }
 
-template <int BN>
-static int launch_tc_persist(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out,
-                             bool relu, cudaStream_t st) {
-    static DeviceOnce once;
-    const int ds = once.slot();
-    if (once.need(ds)) {
-        IRN_CUDA(cudaFuncSetAttribute(conv_tc_persist_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TcPersistCfg<BN>::kSmem));
-        int dev = 0;
-        IRN_CUDA(cudaGetDevice(&dev));
-        IRN_CUDA(cudaDeviceGetAttribute(&once.n_sm[ds], cudaDevAttrMultiProcessorCount, dev));
-        once.done[ds] = true;
-    }
-    const int n_sm = once.n_sm[ds];
-    TcMaps maps;
-    maps.b_hi = BN == 64 && c.bn == 128 ? c.map_bhi64 : c.map_bhi;
-    maps.b_lo = BN == 64 && c.bn == 128 ? c.map_blo64 : c.map_blo;
-    const uint64_t dims[4] = {(uint64_t)c.cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
-    const uint64_t strides[3] = {(uint64_t)c.cin * 4, (uint64_t)W * c.cin * 4, (uint64_t)H * W * c.cin * 4};
-    const uint32_t box[4] = {(uint32_t)kTcBK, (uint32_t)(kTcTW * c.stride), (uint32_t)(kTcTH * c.stride), 1};
-    const uint32_t estr[4] = {1, (uint32_t)c.stride, (uint32_t)c.stride, 1};
-    int rc = make_tensor_map(&maps.a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, in, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
-    if (rc) return rc;
-    TcArgs a;
-    a.bias = c.bias; a.residual = residual; a.out = out;
-    a.B = B; a.Ho = Ho; a.Wo = Wo; a.Cout = c.cout; a.Cin = c.cin; a.ksize = c.k; a.stride = c.stride; a.pad = c.pad;
-    a.relu = relu ? 1 : 0;
-    a.tiles_x = (Wo + kTcTW - 1) / kTcTW;
-    a.tiles_y = (Ho + kTcTH - 1) / kTcTH;
-    a.mode = 0;
-    const long long total = (long long)a.tiles_x * a.tiles_y * B * (c.cout / BN);
-    const unsigned grid = (unsigned)(total < n_sm ? total : n_sm);
-    if (BN == 64 && persist_ts_enabled()) {
-        if ((rc = persist_ts_attr())) return rc;
-        conv_tc_persist_ts_kernel<<<grid, kTcPersistThreads, kPtsSmem, st>>>(maps, a);
-        IRN_LAUNCH_CHECK("conv_tc_persist_ts_kernel");
-        return kOk;
-    }
-    conv_tc_persist_kernel<BN><<<grid, kTcPersistThreads, TcPersistCfg<BN>::kSmem, st>>>(maps, a);
-    IRN_LAUNCH_CHECK("conv_tc_persist_kernel");
-    return kOk;
-}
-
-static int launch_tc_ts(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out, bool relu,
-                        cudaStream_t st) {
-    static DeviceOnce once;
-    const int ds = once.slot();
-    if (once.need(ds)) {
-        IRN_CUDA(cudaFuncSetAttribute(conv_tc_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTsSmem));
-        once.done[ds] = true;
-    }
+// 3xTF32 convolution (eligible when c.bn != 0)
+static int run_conv_tf32(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out, bool relu,
+                         cudaStream_t st) {
     TcMaps maps;
     maps.b_hi = c.map_bhi;
     maps.b_lo = c.map_blo;
-    const uint64_t dims[4] = {(uint64_t)c.cin, (uint64_t)W, (uint64_t)H, (uint64_t)B};
-    const uint64_t strides[3] = {(uint64_t)c.cin * 4, (uint64_t)W * c.cin * 4, (uint64_t)H * W * c.cin * 4};
-    const uint32_t box[4] = {(uint32_t)kTcBK, (uint32_t)(kTcTW * c.stride), (uint32_t)(kTcTH * c.stride), 1};
-    const uint32_t estr[4] = {1, (uint32_t)c.stride, (uint32_t)c.stride, 1};
-    int rc = make_tensor_map(&maps.a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, in, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
+    int rc = act_map(&maps.a, in, B, H, W, c.cin, c.stride);
     if (rc) return rc;
-    TcArgs a;
-    a.bias = c.bias; a.residual = residual; a.out = out;
-    a.B = B; a.Ho = Ho; a.Wo = Wo; a.Cout = c.cout; a.Cin = c.cin; a.ksize = c.k; a.stride = c.stride; a.pad = c.pad;
-    a.relu = relu ? 1 : 0;
-    a.tiles_x = (Wo + kTcTW - 1) / kTcTW;
-    a.tiles_y = (Ho + kTcTH - 1) / kTcTH;
-    a.mode = 0;
-#ifdef IRN_EXPERIMENTAL
-    static const int use_pair = getenv("IRN_TC_PAIR") ? atoi(getenv("IRN_TC_PAIR")) : 0;   // measured: no gain (1322 vs 1323 us on the 3x3x512 layer), kept for A/B
-    if (use_pair) {
-        static DeviceOnce once2;
-        const int ds2 = once2.slot();
-        if (once2.need(ds2)) {
-            IRN_CUDA(cudaFuncSetAttribute(conv_tc_ts2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTsSmem));
-            once2.done[ds2] = true;
-        }
-        maps.b_hi = c.map_bhi64;    // each CTA of a pair loads 64 of the 128 weight rows and multicasts them
-        maps.b_lo = c.map_blo64;
-        const long long m_tiles = (long long)a.tiles_x * a.tiles_y * B;
-        dim3 grid2((unsigned)(((m_tiles + 1) / 2) * (c.cout / 128) * 2));
-        conv_tc_ts2_kernel<<<grid2, kTsThreads, kTsSmem, st>>>(maps, a);
-        IRN_LAUNCH_CHECK("conv_tc_ts2_kernel");
-        return kOk;
-    }
-#endif
-    dim3 grid((unsigned)(a.tiles_x * a.tiles_y * B * (c.cout / 128)));
-    conv_tc_ts_kernel<<<grid, kTsThreads, kTsSmem, st>>>(maps, a);
-    IRN_LAUNCH_CHECK("conv_tc_ts_kernel");
-    return kOk;
+    maps.a2 = maps.a;
+    TcArgs a = conv_args(c, B, Ho, Wo, residual, out, relu);
+    a.oscale = nullptr;
+    return c.bn == 128 ? launch_wg<false, 128>(maps, a, st) : launch_wg<false, 64>(maps, a, st);
 }
 
-// ---- f16x3 kernels (conv_f16.cuh)
-static int f16_mode_flags() {
-    static const int spin = getenv("IRN_F16_SPIN") ? atoi(getenv("IRN_F16_SPIN")) : 1;     // 0: suspending try_wait on the critical path (A/B runs)
-    static const int pf = getenv("IRN_F16_RES_PREFETCH") ? atoi(getenv("IRN_F16_RES_PREFETCH")) : 1;   // 0: no L2 prefetch of the next tile's residual (A/B runs)
-    return (spin ? 0 : 4) | (pf ? 0 : 8);
+// 3xTF32 stem: K = 7 filter rows x (8 taps x 4 channels), out NHWC [B,Ho,Wo,64] with bias + ReLU
+static int launch_tf32_stem(const Conv& c, const float* x4, int B, int Hin, int Win, float* out, cudaStream_t st) {
+    TcMaps maps;
+    maps.b_hi = c.map_bhi;
+    maps.b_lo = c.map_blo;
+    int rc = stem_map(&maps.a, x4, B, Hin, Win);
+    if (rc) return rc;
+    maps.a2 = maps.a;
+    TcArgs a = conv_args(c, B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), nullptr, out, true);
+    a.oscale = nullptr;
+    a.Cin = 32; a.ksize = 7; a.stride = 2; a.pad = 3; a.stem = 1;
+    return launch_wg<false, 64>(maps, a, st);
 }
 
 // Second input of a K-concatenated 1x1 conv (Block::c3ds): NHWC [B, H2, W2, cin2] sampled with pixel stride `stride`
@@ -511,130 +394,38 @@ struct F16Second {
     int H = 0, W = 0, cin = 0, stride = 1;
 };
 
-template <int BN, int NACC, int NSLOT, bool HALO>
-static int launch_f16(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out, bool relu,
-                      cudaStream_t st, const F16Second* second = nullptr) {
-    using Cfg = F16Cfg<BN, NACC, NSLOT>;
-    constexpr size_t smem = HALO ? Cfg::kSmemHalo : Cfg::kSmem;
-    static DeviceOnce once;
-    const int ds = once.slot();
-    if (once.need(ds)) {
-        if (HALO)
-            IRN_CUDA(cudaFuncSetAttribute((conv_f16_halo_kernel<BN, NACC, NSLOT>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        else
-            IRN_CUDA(cudaFuncSetAttribute((conv_f16_kernel<BN, NACC, NSLOT>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int dev = 0;
-        IRN_CUDA(cudaGetDevice(&dev));
-        IRN_CUDA(cudaDeviceGetAttribute(&once.n_sm[ds], cudaDevAttrMultiProcessorCount, dev));
-        once.done[ds] = true;
-    }
-    const int mi = BN == 64 ? 0 : 1;
+// f16x3 convolution (eligible when c.bf_ok)
+static int run_conv_f16(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out, bool relu,
+                        cudaStream_t st, const F16Second* second = nullptr) {
+    const bool wide = c.cout % 128 == 0;
     TcMaps maps;
-    maps.b_hi = c.map_bf_hi[mi];
-    maps.b_lo = c.map_bf_lo[mi];
+    maps.b_hi = c.map_bf_hi[wide ? 1 : 0];
+    maps.b_lo = c.map_bf_lo[wide ? 1 : 0];
     const int cin1 = second ? c.cin - second->cin : c.cin;        // channels of the first input
-    const uint64_t dims[4] = {(uint64_t)cin1, (uint64_t)W, (uint64_t)H, (uint64_t)B};
-    const uint64_t strides[3] = {(uint64_t)cin1 * 4, (uint64_t)W * cin1 * 4, (uint64_t)H * W * cin1 * 4};
-    const uint32_t box[4] = {32u, (uint32_t)(HALO ? kHaloW : kTcTW * c.stride), (uint32_t)(HALO ? kHaloH : kTcTH * c.stride), 1};
-    const uint32_t estr[4] = {1, (uint32_t)(HALO ? 1 : c.stride), (uint32_t)(HALO ? 1 : c.stride), 1};
-    int rc = make_tensor_map(&maps.a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, in, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
+    int rc = act_map(&maps.a, in, B, H, W, cin1, c.stride);
     if (rc) return rc;
     maps.a2 = maps.a;
+    TcArgs a = conv_args(c, B, Ho, Wo, residual, out, relu);
     if (second) {
-        if (HALO || c.k != 1) return fail(kUnsupported, "launch_f16: a second input needs the plain 1x1 kernel");
-        const uint64_t d2[4] = {(uint64_t)second->cin, (uint64_t)second->W, (uint64_t)second->H, (uint64_t)B};
-        const uint64_t s2[3] = {(uint64_t)second->cin * 4, (uint64_t)second->W * second->cin * 4, (uint64_t)second->H * second->W * second->cin * 4};
-        const uint32_t b2[4] = {32u, (uint32_t)(kTcTW * second->stride), (uint32_t)(kTcTH * second->stride), 1};
-        const uint32_t e2[4] = {1, (uint32_t)second->stride, (uint32_t)second->stride, 1};
-        if ((rc = make_tensor_map(&maps.a2, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, second->in, d2, s2, b2, CU_TENSOR_MAP_SWIZZLE_128B, e2))) return rc;
-    }
-    TcArgs a;
-    a.bias = c.bias; a.residual = residual; a.out = out;
-    a.oscale = c.oscale;
-    a.B = B; a.Ho = Ho; a.Wo = Wo; a.Cout = c.cout; a.Cin = c.cin; a.ksize = c.k; a.stride = c.stride; a.pad = c.pad;
-    a.relu = relu ? 1 : 0;
-    a.tiles_x = (Wo + kTcTW - 1) / kTcTW;
-    a.tiles_y = (Ho + kTcTH - 1) / kTcTH;
-    a.mode = f16_mode_flags();
-    if (second) {
+        if (c.k != 1) return fail(kUnsupported, "run_conv_f16: a second input needs a 1x1 conv");
+        if ((rc = act_map(&maps.a2, second->in, B, second->H, second->W, second->cin, second->stride))) return rc;
         a.kb_split = cin1 / kBfBK;
         a.stride2 = second->stride;
     }
-    const long long total = (long long)a.tiles_x * a.tiles_y * B * (c.cout / BN);
-    const int n_sm = once.n_sm[ds];
-    const unsigned grid = (unsigned)(total < n_sm ? total : n_sm);
-    if (HALO) {
-        conv_f16_halo_kernel<BN, NACC, NSLOT><<<grid, kBfThreads, smem, st>>>(maps, a);
-        IRN_LAUNCH_CHECK("conv_f16_halo_kernel");
-    } else {
-        conv_f16_kernel<BN, NACC, NSLOT><<<grid, kBfThreads, smem, st>>>(maps, a);
-        IRN_LAUNCH_CHECK("conv_f16_kernel");
-    }
-    return kOk;
+    return wide ? launch_wg<true, 128>(maps, a, st) : launch_wg<true, 64>(maps, a, st);
 }
 
-// 7x7 / stride-2 stem on the f16x3 kernel: x4 = zero-haloed NHWC4 input [B, Hin+6, Win+8, 4] (as for launch_tc_stem)
+// f16x3 stem: the same rows as the 3xTF32 stem, K = 8 filter rows x 32 (row 7 zero) = four 64-wide k-blocks
 static int launch_f16_stem(const Conv& c, const float* x4, int B, int Hin, int Win, float* out, cudaStream_t st) {
-    using Cfg = F16Cfg<64, 1, 4>;
-    static DeviceOnce once;
-    const int ds = once.slot();
-    if (once.need(ds)) {
-        IRN_CUDA(cudaFuncSetAttribute((conv_f16_kernel<64, 1, 4>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
-        int dev = 0;
-        IRN_CUDA(cudaGetDevice(&dev));
-        IRN_CUDA(cudaDeviceGetAttribute(&once.n_sm[ds], cudaDevAttrMultiProcessorCount, dev));
-        once.done[ds] = true;
-    }
-    const int Hp = Hin + 6, Wp = Win + 8;
-    const int Ho = conv_out(Hin, 7, 2, 3), Wo = conv_out(Win, 7, 2, 3);
     TcMaps maps;
     maps.b_hi = c.map_bf_hi[0];
     maps.b_lo = c.map_bf_lo[0];
-    // dim0: the 32 contiguous floats (8 px x 4 ch) of one filter-row window; dim1: output column (windows overlap: stride 2 px = 32 B);
-    // dim2: padded input row; dim3: image
-    const uint64_t dims[4] = {32, (uint64_t)Wo, (uint64_t)Hp, (uint64_t)B};
-    const uint64_t strides[3] = {32, (uint64_t)Wp * 16, (uint64_t)Hp * Wp * 16};
-    const uint32_t box[4] = {32, (uint32_t)kTcTW, (uint32_t)(kTcTH * 2), 1};
-    const uint32_t estr[4] = {1, 1, 2, 1};
-    int rc = make_tensor_map(&maps.a, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
+    int rc = stem_map(&maps.a, x4, B, Hin, Win);
     if (rc) return rc;
     maps.a2 = maps.a;
-    TcArgs a;
-    a.bias = c.bias; a.residual = nullptr; a.out = out;
-    a.oscale = c.oscale;
-    a.B = B; a.Ho = Ho; a.Wo = Wo; a.Cout = 64; a.Cin = 256; a.ksize = 1; a.stride = 2; a.pad = 0; a.relu = 1;
-    a.tiles_x = (Wo + kTcTW - 1) / kTcTW;
-    a.tiles_y = (Ho + kTcTH - 1) / kTcTH;
-    a.mode = f16_mode_flags() | 1;
-    const long long total = (long long)a.tiles_x * a.tiles_y * B;
-    const int n_sm = once.n_sm[ds];
-    conv_f16_kernel<64, 1, 4><<<(unsigned)(total < n_sm ? total : n_sm), kBfThreads, Cfg::kSmem, st>>>(maps, a);
-    IRN_LAUNCH_CHECK("conv_f16_kernel(stem)");
-    return kOk;
-}
-
-// f16x3 dispatch.  Reductions with K >= 512 keep the hi*hi and the cross terms in separate TMEM accumulators (the tensor core's
-// accumulate truncates: conv_f16.cuh, f16_issue3), shorter ones use one accumulator per tile and two accumulator sets so that the
-// epilogue of a tile overlaps the next tile's mainloop (they are memory-bound).  3x3 / stride 1 convs take the halo-tile kernel.
-template <bool HALO>
-static int dispatch_f16(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out, bool relu,
-                        cudaStream_t st, const F16Second* second = nullptr) {
-    const int K = c.k * c.k * c.cin;
-    static const int acc_min_k = getenv("IRN_F16_ACC_MINK") ? atoi(getenv("IRN_F16_ACC_MINK")) : 512;
-    const bool sep = K >= acc_min_k;
-    if (c.cout % 128 == 0) {
-        if (sep) return launch_f16<128, 2, 4, HALO>(c, in, B, H, W, Ho, Wo, residual, out, relu, st, second);
-        return launch_f16<128, 1, 4, HALO>(c, in, B, H, W, Ho, Wo, residual, out, relu, st, second);
-    }
-    if (sep) return launch_f16<64, 2, 4, HALO>(c, in, B, H, W, Ho, Wo, residual, out, relu, st, second);
-    return launch_f16<64, 1, 4, HALO>(c, in, B, H, W, Ho, Wo, residual, out, relu, st, second);
-}
-
-static int run_conv_bf16(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out, bool relu,
-                         cudaStream_t st) {
-    static const int use_halo = getenv("IRN_F16_HALO") ? atoi(getenv("IRN_F16_HALO")) : 1;
-    if (use_halo && c.k == 3 && c.stride == 1 && c.pad == 1) return dispatch_f16<true>(c, in, B, H, W, Ho, Wo, residual, out, relu, st);
-    return dispatch_f16<false>(c, in, B, H, W, Ho, Wo, residual, out, relu, st);
+    TcArgs a = conv_args(c, B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), nullptr, out, true);
+    a.Cin = 256; a.ksize = 1; a.stride = 2; a.pad = 0; a.stem = 1;
+    return launch_wg<true, 64>(maps, a, st);
 }
 
 static int run_conv(const irn_net* net, const Conv& c, const float* in, int B, int H, int W, const float* residual, float* out, bool relu,
@@ -646,23 +437,8 @@ static int run_conv(const irn_net* net, const Conv& c, const float* in, int B, i
     g.Cout = c.cout; g.k = c.k; g.stride = c.stride; g.pad = c.pad;
     if (Ho_) *Ho_ = g.Ho;
     if (Wo_) *Wo_ = g.Wo;
-    if (net->conv_mode == 2 && c.bf_ok) return run_conv_bf16(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
-    if (net->conv_mode >= 1 && c.bn) {
-        // short reductions (K <= 256) are latency-bound per tile: 64-wide tiles with a 2-stage pipeline and two TMEM
-        // accumulators let two CTAs share an SM; long reductions use the 3-stage, 3-accumulator configuration
-        const int K = c.k * c.k * c.cin;
-        static const int persist_max_k = getenv("IRN_TC_PERSIST_MAXK") ? atoi(getenv("IRN_TC_PERSIST_MAXK")) : 640;
-        if (K <= persist_max_k) {   // persistent, epilogue-overlapped kernel for the short reductions
-            if (c.bn == 128) return launch_tc_persist<128>(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
-            return launch_tc_persist<64>(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
-        }
-        if (K <= 128) return launch_tc<64, 2, 2>(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
-        if (K <= 256) return launch_tc<64, 2, 3>(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
-        static const int use_ts = getenv("IRN_TC_TS") ? atoi(getenv("IRN_TC_TS")) : 1;
-        if (c.bn == 128 && use_ts) return launch_tc_ts(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);   // A operand from TMEM
-        if (c.bn == 128) return launch_tc<128, 3, 3>(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
-        return launch_tc<64, 3, 3>(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
-    }
+    if (net->conv_mode == 2 && c.bf_ok) return run_conv_f16(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
+    if (net->conv_mode >= 1 && c.bn) return run_conv_tf32(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
     const int M = B * g.Ho * g.Wo;
     dim3 grid((M + kBM - 1) / kBM, (c.cout + kBN - 1) / kBN);
     if (c.cin % 16 == 0)
@@ -735,7 +511,7 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
         static const int stem_f16 = getenv("IRN_F16_STEM") ? atoi(getenv("IRN_F16_STEM")) : 1;
         if (net->conv_mode == 2 && net->stem_f16.bf_ok && stem_f16) {
             if ((rc = launch_f16_stem(net->stem_f16, x_in, B, Hin, Win, stem_out, st))) return rc;
-        } else if ((rc = launch_tc_stem(net->stem, x_in, B, Hin, Win, stem_out, st))) return rc;
+        } else if ((rc = launch_tf32_stem(net->stem, x_in, B, Hin, Win, stem_out, st))) return rc;
     } else {
         const size_t total = (size_t)B * Hin * Win * 3;
         nchw_to_nhwc_pad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, x_in, B, 3, H, W, Hin, Win);
@@ -775,7 +551,7 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
             if (fused) {   // conv3 + projection shortcut in one reduction: [t2 ; x sampled at the block's stride]
                 F16Second sec;
                 sec.in = x; sec.H = h; sec.W = w; sec.cin = blk.ds.cin; sec.stride = blk.ds.stride;
-                if ((rc = dispatch_f16<false>(blk.c3ds, t2, B, ho, wo, ho, wo, nullptr, out, true, st, &sec))) return rc;
+                if ((rc = run_conv_f16(blk.c3ds, t2, B, ho, wo, ho, wo, nullptr, out, true, st, &sec))) return rc;
             } else if ((rc = run_conv(net, blk.c3, t2, B, ho, wo, res, out, true, st, nullptr, nullptr))) return rc;   // out += residual; relu (net/resnet50.py:51-52)
             x = out;
             h = ho;
@@ -841,7 +617,7 @@ extern "C" int irn_conv_forward(irn_conv* c, const float* in, int B, int H, int 
 }
 
 extern "C" int irn_net_set_conv_mode(irn_net* net, int mode) {
-    if (!net || mode < 0 || mode > 2) return fail(kBadArg, "irn_net_set_conv_mode: mode must be 0 (SIMT fp32), 1 (tcgen05 3xTF32) or 2 (tcgen05 f16x3)");
+    if (!net || mode < 0 || mode > 2) return fail(kBadArg, "irn_net_set_conv_mode: mode must be 0 (SIMT fp32), 1 (wgmma 3xTF32) or 2 (wgmma f16x3)");
     net->conv_mode = mode;
     return kOk;
 }

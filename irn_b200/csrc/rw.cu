@@ -439,7 +439,7 @@ rw_step_tma_kernel(const __grid_constant__ RwMaps maps, const double* __restrict
     }
 }
 
-#ifdef IRN_EXPERIMENTAL   // persistent ring variant of the per-step kernel: measured slower (profiles/r01_rw_experiments.md); not in the product build
+#ifdef IRN_EXPERIMENTAL   // persistent ring variant of the per-step kernel: an experiment, not in the product build
 // ---------------------------------------------------------------- persistent ring step kernel (radius 5, experiment, variant 3)
 // Same arithmetic as rw_step_tma_kernel, restructured so that TMA latency is never exposed: one persistent CTA per SM
 // walks tiles b, b+G, b+2G, ...; warp 4 is a TMA producer that runs ahead through a ring of kRingW weight-class buffers and
@@ -974,19 +974,20 @@ static int walk_impl(const float* x, const float* edge, float* out, int n_img, c
     int n_fused_clusters = 0;
     bool want_fused = radius == 5 && (variant == 0 || variant == 4 || variant == 5) && h <= kFR * 16 && w <= kFW;
     if (want_fused && variant == 0) {
-        // Both kernels give bit-identical results; pick the faster one from B200 measurements (profiles/r01_rw_fused.md):
-        // the fused kernel walks one (image, class) per cluster at ~2.85 us per step on the ~7 clusters that fit; the per-step
-        // kernel shares the weight reads between up to 4 classes of an image (~0.54 + 0.15 C us per image-chunk per step once
-        // the grid fills the GPU, ~9 us per step at least).  Single-class images favour the fused kernel, large batches of
-        // many-class images (instance path: classes x instances) the per-step one.
+        // Both kernels give bit-identical results; pick the faster one from a cost model fitted to H100 measurements
+        // (tools/rw_micro.py, variants 2 and 4, 128x128 grids, 1-4 classes per image): the fused kernel walks one (image, class)
+        // per cluster at ~3.0 us per step on the 7 clusters of 16 CTAs that fit; the per-step kernel shares the weight reads
+        // between up to 4 classes of an image (~1.13 + 0.22 C us per image-chunk per step, ~10 us per step at least).
+        // Single-class images favour the fused kernel, large batches of many-class images (instance path: classes x
+        // instances) the per-step one.
         double step_us = 0.0;
         for (int i = 0; i < n_img; ++i) {
             int c = chan_offsets[i + 1] - chan_offsets[i];
-            for (; c > 0; c -= 4) step_us += 0.54 + 0.15 * (c < 4 ? c : 4);
+            for (; c > 0; c -= 4) step_us += 1.13 + 0.22 * (c < 4 ? c : 4);
         }
         step_us *= (double)h * w / (128.0 * 128.0);
-        if (step_us < 9.0) step_us = 9.0;
-        const double fused_us = 2.85 * ((totc + 6) / 7);
+        if (step_us < 10.0) step_us = 10.0;
+        const double fused_us = 3.0 * ((totc + 6) / 7);
         want_fused = fused_us <= step_us;
     }
     if (want_fused) {

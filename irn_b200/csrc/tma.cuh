@@ -1,4 +1,4 @@
-// TMA (cp.async.bulk.tensor) + mbarrier helpers for sm_100a, and the host-side tensor-map
+// TMA (cp.async.bulk.tensor) + mbarrier helpers for sm_90a, and the host-side tensor-map
 // encoder (driver entry point resolved at run time: libirn_b200.so does not link libcuda).
 #pragma once
 #include <cuda.h>

@@ -1,4 +1,4 @@
-"""Drop-in for the reference's ``misc/indexing.py`` on B200.
+"""Drop-in for the reference's ``misc/indexing.py`` on H100.
 
 Same names, argument meaning and return layout as the reference (misc/indexing.py:6-167):
 ``PathIndex`` (identical public attributes, built by the C ABI on the host, integer

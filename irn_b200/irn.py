@@ -25,7 +25,7 @@ class EdgeDisplacement(IrnParams):
         self._conv_mode = None
 
     def set_conv_mode(self, mode):
-        """0 SIMT fp32, 1 tcgen05 3xTF32 (default: the edge head needs it for the 1e-4 contract), 2 tcgen05 bf16x3."""
+        """0 SIMT fp32, 1 wgmma 3xTF32, 2 wgmma f16x3 (default)."""
         self._conv_mode = None if mode is None else int(mode)
         if self._plan is not None and self._conv_mode is not None:
             _lib.check(_lib.lib().irn_net_set_conv_mode(self._plan.handle, self._conv_mode), "irn_net_set_conv_mode")

@@ -9,7 +9,7 @@ from . import _lib
 
 class Conv2d:
     """conv (+ folded FixedBatchNorm) -> [+ residual] -> [ReLU] on NHWC fp32 CUDA tensors
-    (net/resnet50.py:34-54 building block).  mode 0 = SIMT fp32, 1 = tcgen05 3xTF32."""
+    (net/resnet50.py:34-54 building block).  mode 0 = SIMT fp32, 1 = wgmma 3xTF32, 2 = wgmma f16x3."""
 
     def __init__(self, weight_oihw, bn=None, stride=1, pad=0):
         w = np.ascontiguousarray(weight_oihw, dtype=np.float32)

@@ -48,8 +48,8 @@ LOADER_CHUNK = 8
 def collate_chunk(batch):
     """Several consecutive items as ONE message from a loader worker: the decoded images (or JPEG byte streams) in one flat uint8
     tensor, the stored CAMs in one flat fp32 tensor.  A DataLoader hands every tensor of every item to the main process through its
-    own file-descriptor exchange (~0.5 ms each): with batch_size=1 and five tensors per item that alone capped the label steps at
-    ~400 images/s on the B200 host, whatever the number of workers (profiles/r02_config4_loader.md).  `split_chunk` turns the
+    own file-descriptor exchange (~0.5 ms each): with batch_size=1 and five tensors per item that alone caps the label steps at a
+    few hundred images/s, whatever the number of workers.  `split_chunk` turns the
     message back into batch_size=1 packs (views, no copies)."""
     out = {"names": [b["name"] for b in batch], "sizes": [(int(b["size"][0]), int(b["size"][1])) for b in batch],
            "label": torch.stack([torch.as_tensor(b["label"]) for b in batch])}
@@ -303,9 +303,9 @@ class StepContext:
 def threaded_loader(shard, n_threads, prefetch):
     """Items of `shard` in order, collated like the batch-size-1 DataLoader, produced by a thread pool instead of forked worker
     processes: PIL's JPEG decoder and the file reads release the GIL, and a thread hands its arrays over without the
-    shared-memory copy -- and without the ~1 s it takes to fork a dozen workers off a process that holds a CUDA context.  MEASURED
-    SLOWER than the forked workers on the B200 host (the unpickling of the CAM dicts, numpy copies and collation serialise on the
-    GIL: sem-seg pass 9.5 s against 3.1 s), so it is opt-in (--loader_threads True) and kept for hosts where fork is the problem."""
+    shared-memory copy -- and without the ~1 s it takes to fork a dozen workers off a process that holds a CUDA context.  Usually
+    slower than the forked workers (the unpickling of the CAM dicts, numpy copies and collation serialise on the GIL), so it is
+    opt-in (--loader_threads True) and kept for hosts where fork is the problem."""
     from collections import deque
     n = len(shard)
     with ThreadPoolExecutor(max_workers=max(1, n_threads)) as pool:
@@ -345,7 +345,7 @@ def work_loop(process_id, model, dataset, args, per_image, per_batch=None):
             return
         ctx = StepContext(model, args, torch.device("cuda", process_id), scales)
         chunked = True
-        if getattr(args, "loader_threads", False):     # measured slower than forked workers (GIL: 82 vs 148 images/s, bench --config 4): off
+        if getattr(args, "loader_threads", False):     # slower than forked workers (GIL): off
             loader, chunked = threaded_loader(shard, max(2, args.num_workers // n_gpus), prefetch=2 * bsz), False
         buckets = {}
         prof = os.environ.get("IRN_STEP_PROFILE")          # host-side time split of the loop (development aid), printed to stderr
@@ -417,8 +417,8 @@ def to_device_list(ctx, tensors):
     per image)."""
     counts = [int(t.shape[0]) for t in tensors]
     # through PINNED memory (torch's caching host allocator keeps the block alive until the copy has run): a copy from pageable memory
-    # is staged in stream order, i.e. the host would sit here until the GPU has finished everything issued before it -- measured
-    # 1.0 s of a 2.3 s sem-seg pass waiting for the IRNet forward of the same bucket (profiles/r02_config4_loader.md)
+    # is staged in stream order, i.e. the host would sit here until the GPU has finished everything issued before it (the IRNet
+    # forward of the same bucket)
     staged = torch.empty((sum(counts),) + tuple(tensors[0].shape[1:]), dtype=torch.float32, pin_memory=True)
     torch.cat([torch.as_tensor(t).float() for t in tensors], 0, out=staged)
     dev = staged.to(ctx.device, non_blocking=True)

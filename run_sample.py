@@ -6,7 +6,7 @@ so the reference's evaluation steps (step/eval_cam.py, step/eval_sem_seg.py, ste
 ``result/cam/*.npy``, ``result/sem_seg/*.png`` and ``result/ins_seg/*.npy`` unchanged.  Only the three hot-path steps
 run here (make_cam, make_ins_seg_labels, make_sem_seg_labels); training / CRF / evaluation passes are the reference's own.
 
-Differences: --cam_network / --irn_network default to the B200 modules; flags the reference declares without a type
+Differences: --cam_network / --irn_network default to the irn_b200 modules; flags the reference declares without a type
 (--beta, --exp_times, --*_bg_thres, --*_pass) are parsed; --synthetic N runs on N seeded synthetic images instead of VOC
 (--synthetic_list names them); --step_batch N images of equal size are processed together (1 = the reference's loop).
 """
@@ -76,7 +76,7 @@ def main(argv=None):
             importlib.import_module("irn_b200.step." + EVAL_STEPS[name]).run(args)
             continue
         if name not in HOT_STEPS:
-            print("[irn_b200] step.%s is outside the B200 hot path: run the reference's own step for it" % name)
+            print("[irn_b200] step.%s is outside the native hot path: run the reference's own step for it" % name)
             continue
         module = importlib.import_module("irn_b200.step." + HOT_STEPS[name])
         pyutils.Timer("step.%s:" % HOT_STEPS[name])

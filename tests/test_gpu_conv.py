@@ -1,4 +1,4 @@
-"""The convolution kernels (SIMT fp32 and tcgen05 3xTF32) against a plain torch fp32 reference of the same
+"""The convolution kernels (SIMT fp32 and wgmma 3xTF32) against a plain torch fp32 reference of the same
 op (F.conv2d + batch_norm on the GPU with TF32 disabled)."""
 import pytest
 import torch
@@ -11,13 +11,13 @@ pytestmark = pytest.mark.gpu
 CASES = [  # cin, cout, k, stride, pad, B, H, W
     (64, 256, 1, 1, 0, 2, 40, 48),
     (64, 64, 3, 1, 1, 2, 37, 53),      # ragged tiles
-    (64, 64, 3, 1, 1, 4, 128, 160),    # 640 tiles: several per persistent CTA (both accumulator sets, ring wrap-around)
-    (256, 64, 1, 1, 0, 4, 96, 128),    # 8 k-blocks per tile through the 5-stage ring, A operand from TMEM
-    (64, 256, 1, 1, 0, 4, 96, 128),    # 768 tiles through the shared-memory-operand persistent kernel
+    (64, 64, 3, 1, 1, 4, 128, 160),    # 640 tiles, 18 k-blocks each
+    (256, 64, 1, 1, 0, 4, 96, 128),    # 8 k-blocks per tile: ring wrap-around
+    (64, 256, 1, 1, 0, 4, 96, 128),    # 768 tiles
     (128, 128, 3, 2, 1, 2, 64, 64),
     (256, 512, 1, 2, 0, 2, 33, 47),
     (512, 128, 1, 1, 0, 3, 16, 16),
-    (512, 512, 3, 1, 1, 2, 20, 24),    # K = 4608: A-from-TMEM kernel
+    (512, 512, 3, 1, 1, 2, 20, 24),    # K = 4608: 144 k-blocks
     (1024, 256, 1, 1, 0, 2, 33, 17),
     (2048, 512, 1, 1, 0, 1, 16, 16),
     (3, 64, 7, 2, 3, 2, 64, 80),       # stem: SIMT only
@@ -50,30 +50,30 @@ def test_conv_vs_torch(cuda_dev, case):
     if cin % 32 == 0 and cout % 64 == 0 and k in (1, 3):
         y1 = conv(x_nhwc, res_nhwc, relu=True, mode=1)
         err = (y1 - ref).abs().max().item() / scale
-        assert err < 1e-5, "tcgen05 3xTF32 rel err %g" % err   # tensor-core fp32 accumulation truncates; see conv_tc.cuh
+        assert err < 1e-5, "wgmma 3xTF32 rel err %g" % err   # tensor-core fp32 accumulation truncates; see conv_wgmma.cuh
         print("tc err", case, err)
 
 
 F16_CASES = [  # cin, cout, k, stride, pad, B, H, W, residual   (f16x3 kernel: Cin % 64 == 0, Cout % 64 == 0)
     (64, 64, 1, 1, 0, 2, 40, 48, False),       # N tile 64, one k-block per tile
-    (64, 64, 3, 1, 1, 4, 128, 160, False),     # N tile 64, 9 k-blocks, 640 tiles: ring wrap-around, both accumulator sets
+    (64, 64, 3, 1, 1, 4, 128, 160, False),     # N tile 64, 9 k-blocks, 640 tiles: ring wrap-around
     (64, 256, 1, 1, 0, 4, 96, 128, True),      # N tile 128 + residual (K < 512)
     (256, 64, 1, 1, 0, 2, 37, 53, False),      # ragged tiles
     (128, 128, 3, 2, 1, 2, 64, 64, False),     # stride-2 3x3
     (128, 512, 1, 1, 0, 2, 33, 47, True),
     (256, 512, 1, 2, 0, 2, 33, 47, False),     # stride-2 projection, K = 256: N tile 128
-    (512, 1024, 1, 2, 0, 2, 32, 32, False),    # K = 512, no residual: N tile 256
-    (256, 256, 3, 1, 1, 3, 32, 32, False),     # K = 2304: N tile 256, one N tile per pixel tile
-    (512, 512, 3, 1, 1, 2, 20, 24, False),     # K = 4608: 72 k-blocks into one accumulator
-    (512, 2048, 1, 1, 0, 2, 16, 16, True),     # residual -> N tile 128 although K = 512
+    (512, 1024, 1, 2, 0, 2, 32, 32, False),    # K = 512, no residual
+    (256, 256, 3, 1, 1, 3, 32, 32, False),     # K = 2304
+    (512, 512, 3, 1, 1, 2, 20, 24, False),     # K = 4608: 72 k-blocks
+    (512, 2048, 1, 1, 0, 2, 16, 16, True),     # residual, N tile 128
     (1024, 256, 1, 1, 0, 2, 33, 17, False),
-    (2048, 512, 1, 1, 0, 5, 16, 16, False),    # several tiles per CTA with the single accumulator set of the 256-wide tile
+    (2048, 512, 1, 1, 0, 5, 16, 16, False),    # K = 2048, 5 images
 ]
 
 
 @pytest.mark.parametrize("case", F16_CASES, ids=lambda c: "x".join(map(str, c)))
 def test_conv_f16x3_vs_torch(cuda_dev, case):
-    """conv_f16_kernel (mode 2: fp16 hi/lo split operands, fp32 accumulation) against fp64 torch.  Same tolerance as the 3xTF32
+    """conv_wg_kernel<f16x3> (mode 2: fp16 hi/lo split operands, fp32 accumulation) against fp64 torch.  Same tolerance as the 3xTF32
     kernels: fp16 and tf32 carry the same 11 significant bits, the split keeps ~22 per operand."""
     from conftest import record
     cin, cout, k, stride, pad, B, H, W, with_res = case

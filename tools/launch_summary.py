@@ -23,7 +23,7 @@ def load(path):
 
 def key(n):
     k = re.sub(r"<.*", "", n.split("(")[0]).replace("void ", "").replace("irn::", "")
-    m = re.search(r"(conv_tc\w*kernel)(<[^>]*>)?", n)
+    m = re.search(r"(conv_wg\w*kernel)(<[^>]*>)?", n)
     if m:
         k = m.group(1) + (m.group(2) or "")
     return k

@@ -43,10 +43,10 @@ def main(path, skip=0):
     for k, (t, w, b, c) in sorted(fam.items(), key=lambda kv: -kv[1][0]):
         print("%-44s %10.1f %6.1f%% %7d %10.1f %9.1f" % (k, t, 100 * t / tot_t, c, w / t if t else 0, b / 1e6))
     print("%-44s %10.1f %6.1f%% %7s %10.1f %9.1f   <- time-weighted tensor-pipe %% over all launches" % ("TOTAL", tot_t, 100.0, "", tot_w / tot_t, tot_b / 1e6))
-    conv_t = sum(v[0] for k, v in fam.items() if k.startswith(("conv_tc", "conv_f16")))
-    conv_w = sum(v[1] for k, v in fam.items() if k.startswith(("conv_tc", "conv_f16")))
+    conv_t = sum(v[0] for k, v in fam.items() if k.startswith("conv_wg"))
+    conv_w = sum(v[1] for k, v in fam.items() if k.startswith("conv_wg"))
     if conv_t:
-        print("tcgen05 conv kernels only: %.1f us, time-weighted tensor pipe %.1f %%" % (conv_t, conv_w / conv_t))
+        print("wgmma conv kernels only: %.1f us, time-weighted tensor pipe %.1f %%" % (conv_t, conv_w / conv_t))
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""Print the key metrics of an .ncu-rep (development aid; output is what gets copied into profiles/)."""
+"""Print the key metrics of an .ncu-rep (development aid)."""
 import csv, subprocess, sys
 KEYS = ['gpu__time_duration.sum', 'dram__bytes_read.sum', 'dram__bytes_write.sum', 'gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed',
         'lts__t_bytes.sum', 'lts__t_sector_hit_rate.pct', 'l1tex__t_sector_hit_rate.pct', 'sm__throughput.avg.pct_of_peak_sustained_elapsed',

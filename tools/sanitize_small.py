@@ -1,5 +1,5 @@
 """Small-shape tour of every hand-written kernel family, meant to run under compute-sanitizer (memcheck / racecheck /
-initcheck): fused cluster walk at every cluster size 1..16, the per-step walk, the tcgen05 convolution kernels (3xTF32 and
+initcheck): fused cluster walk at every cluster size 1..16, the per-step walk, the wgmma convolution kernels (3xTF32 and
 bf16x3, every N tile), labels, CAM merge, instance kernels, input pyramids.
     compute-sanitizer --tool memcheck python tools/sanitize_small.py"""
 import os
@@ -23,7 +23,7 @@ for h, w in [(8, 40), (16, 33), (30, 64), (60, 50), (128, 128)]:
     torch.cuda.synchronize()
     print("walk", h, w, "ok", flush=True)
 
-# convolutions: (cin, cout, k, stride, H, W, residual) -> every tcgen05 kernel family once
+# convolutions: (cin, cout, k, stride, H, W, residual) -> every wgmma kernel configuration once
 for cin, cout, k, s, H, W, res in [(64, 64, 3, 1, 20, 24, False), (64, 256, 1, 1, 20, 24, True), (256, 64, 1, 1, 20, 24, False),
                                    (128, 128, 3, 2, 24, 24, False), (256, 256, 3, 1, 16, 16, False), (1024, 256, 1, 1, 16, 16, False),
                                    (512, 1024, 1, 2, 16, 16, False)]:
