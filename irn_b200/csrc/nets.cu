@@ -316,13 +316,21 @@ static inline int conv_out(int n, int k, int s, int p) { return (n + 2 * p - k) 
 template <bool F16, int BN>
 static int launch_wg(const TcMaps& maps, const TcArgs& a, cudaStream_t st) {
     using Cfg = WgCfg<F16, BN>;
-    static DeviceOnce once;
+    static DeviceOnce once;   // n_sm[] holds the number of co-resident CTAs of the device
     const int ds = once.slot();
     if (once.need(ds)) {
         IRN_CUDA(cudaFuncSetAttribute((conv_wg_kernel<F16, BN>), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::kSmem));
+        int dev = 0, n_sm = 0, per_sm = 0;
+        IRN_CUDA(cudaGetDevice(&dev));
+        IRN_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+        IRN_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv_wg_kernel<F16, BN>, kWgThreads, Cfg::kSmem));
+        if (per_sm < 1) return fail(kCudaError, "conv_wg_kernel: no CTA fits on an SM (%zu bytes of shared memory)", Cfg::kSmem);
+        once.n_sm[ds] = n_sm * per_sm;
         once.done[ds] = true;
     }
-    const long long grid = (long long)a.tiles_x * a.tiles_y * a.B * (a.Cout / BN);
+    // persistent CTAs: each walks the work items (spatial tile x N tile) with stride gridDim.x
+    const long long items = (long long)a.tiles_x * a.tiles_y * a.B * (a.Cout / BN);
+    const long long grid = items < once.n_sm[ds] ? items : once.n_sm[ds];
     conv_wg_kernel<F16, BN><<<(unsigned)grid, kWgThreads, Cfg::kSmem, st>>>(maps, a);
     IRN_LAUNCH_CHECK(F16 ? "conv_wg_kernel<f16x3>" : "conv_wg_kernel<3xtf32>");
     return kOk;
