@@ -263,6 +263,37 @@ int irn_jpeg_image_size(irn_jpeg* decoder, const uint8_t* data, size_t length, i
 int irn_jpeg_decode_batch(irn_jpeg* decoder, const uint8_t* const* data, const size_t* lengths, int n, uint8_t* out_dev,
                           int H, int W, irn_stream_t stream);
 
+/* ------------------------------------------------------------------------------------
+ * N3  fully connected CRF and the cam_to_ir_label step.  Replaces misc/imutils.py:156-170 (crf_inference_label: pydensecrf's
+ * DenseCRF2D with a Gaussian (sxy) and a bilateral (sxy, srgb) Potts term, mean-field inference on the permutohedral lattice)
+ * and the body of step/cam_to_ir_label.py:19-41.  The arithmetic is oracle/crf.py's (float32, fixed evaluation order, no
+ * floating-point atomics: bitwise reproducible).  A batch is n images of one size; images uint8 [n,H,W,3] (RGB, HWC).
+ *
+ * irn_crf_workspace_bytes  device workspace for n images with n_groups CRFs each (1: irn_dense_crf, 2: irn_ir_label) of at most
+ *                         max_labels labels (<= irn_crf_max_labels()); 0 for arguments no call accepts.
+ * irn_dense_crf           labels int32 [n,H,W] in [0, n_labels) -> labels_out int32 [n,H,W] = argmax of Q after t iterations,
+ *                         q_out fp32 [n,n_labels,H,W] = Q (either may be NULL, not both); unary from the labels with gt_prob
+ *                         (pydensecrf.utils.unary_from_labels, zero_unsure=False).  A label outside [0, n_labels) -> -1.
+ * irn_ir_label            high_res fp32 [sum(counts),H,W] (make_cam's high_res planes, images back to back), keys_host HOST int32
+ *                         [sum(counts)] (make_cam's keys), counts_host HOST int32 [n] -> out uint8 [n,H,W]: the conf map of the
+ *                         step (fg / bg confident maps through the CRF, t=10, gt_prob=0.7, Gaussian (3, compat 3), bilateral
+ *                         (50, 5, compat 10); 0 = bg, 255 = unsure, else class + 1).  An image with no class is all 0.
+ * vertex_counts           optional HOST int32 [n,2]: lattice vertices per image (Gaussian, bilateral).
+ * Both synchronise the stream once, after the lattice build (vertex counts and argument errors reach the host there).
+ * irn_crf_set_timing / irn_crf_last_ms: CUDA events around the build, the iterations and the tail of the next calls on this
+ * thread; last_ms waits and returns the three durations of the last timed call (ms).
+ */
+size_t irn_crf_workspace_bytes(int n, int H, int W, int n_groups, int max_labels);
+int irn_crf_max_labels(void);
+int irn_dense_crf(const uint8_t* img, const int32_t* labels, int n, int H, int W, int n_labels, int t, double gt_prob,
+                  float gauss_sxy, float gauss_compat, float bil_sxy, float bil_srgb, float bil_compat, int32_t* labels_out,
+                  float* q_out, int32_t* vertex_counts, void* workspace, size_t workspace_bytes, irn_stream_t stream);
+int irn_ir_label(const uint8_t* img, const float* high_res, const int32_t* keys_host, const int32_t* counts_host, int n, int H,
+                 int W, float conf_fg_thres, float conf_bg_thres, uint8_t* out, int32_t* vertex_counts, void* workspace,
+                 size_t workspace_bytes, irn_stream_t stream);
+int irn_crf_set_timing(int enable);
+int irn_crf_last_ms(float* ms3);
+
 #ifdef __cplusplus
 }
 #endif

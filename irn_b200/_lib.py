@@ -69,6 +69,14 @@ SIGNATURES = {
     "irn_resize_plan_destroy": (c_int, [c_void_p]),
     "irn_resize_workspace_bytes": (c_size_t, [c_void_p, c_int]),
     "irn_resize_forward": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "irn_crf_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "irn_crf_max_labels": (c_int, []),
+    "irn_dense_crf": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_float, c_float, c_float, c_float,
+                              c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "irn_ir_label": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p,
+                             c_void_p, c_size_t, c_void_p]),
+    "irn_crf_set_timing": (c_int, [c_int]),
+    "irn_crf_last_ms": (c_int, [ctypes.POINTER(c_float)]),
 }
 
 

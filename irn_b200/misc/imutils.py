@@ -36,3 +36,16 @@ def compress_range(arr):
 
 def HWC_to_CHW(img):
     return np.transpose(img, (2, 0, 1))
+
+
+def crf_inference_label(img, labels, t=10, n_labels=21, gt_prob=0.7):
+    """misc/imutils.py:156-170: the dense CRF (Gaussian sxy=3 compat=3, bilateral sxy=50 srgb=5 compat=10, t mean-field
+    iterations) of uint8 [H,W,3] `img` with the unary of the label map `labels` [H,W], argmax over labels.  numpy in, numpy out
+    (int64 [H,W]); computed on the current CUDA device (irn_b200.crf).  n_labels == 1 gives label 0 everywhere."""
+    import torch
+    from .. import crf
+    dev = torch.device("cuda", torch.cuda.current_device())
+    x = torch.from_numpy(np.ascontiguousarray(img, dtype=np.uint8))[None].to(dev)
+    lab = torch.from_numpy(np.ascontiguousarray(labels, dtype=np.int32))[None].to(dev)
+    out, _, _ = crf.dense_crf(x, lab, n_labels, t=t, gt_prob=gt_prob)
+    return out[0].cpu().numpy().astype(np.int64)

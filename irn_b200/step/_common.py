@@ -114,20 +114,24 @@ def step_batch(args):
     return max(1, int(getattr(args, "step_batch", DEFAULT_STEP_BATCH) or 1))
 
 
-def make_dataset(args, list_path, scales, cam_dir=None):
+def make_dataset(args, list_path, scales, cam_dir=None, cam_field="cam", raw_images=False):
     """VOC images from --voc12_root, or seeded synthetic ones with --synthetic N.  `cam_dir`: the label steps let the loader
-    workers read the stored CAM dicts (batched mode only; the one-image loop reads them itself, like the reference)."""
-    if step_batch(args) == 1 or not device_pyramid(args):
+    workers read the stored CAM dicts (batched mode only; the one-image loop reads them itself, like the reference), and ship
+    their `cam_field` map.  `raw_images`: a step without a network takes the decoded uint8 images themselves (host decode, as
+    the reference's VOC12ImageDataset with img_normal=None), whatever --device_pyramid / --device_jpeg say."""
+    if step_batch(args) == 1 or not (device_pyramid(args) or raw_images):
         cam_dir = None
+    decode_only = True if raw_images else device_pyramid(args)
     if getattr(args, "synthetic", 0):
         # one id list for ALL steps (the reference reads --train_list in make_cam but --infer_list in the label steps; with
         # synthetic images the later steps must find the .npy files the first one wrote): --synthetic_list, else 2007_%06d
         names = getattr(args, "synthetic_list", None) or None
         if names is not None and not os.path.exists(names):
             raise FileNotFoundError("--synthetic_list %s" % names)
-        return voc_data.SyntheticMSF(int(args.synthetic), scales=scales, name_list=names, decode_only=device_pyramid(args), cam_dir=cam_dir)
-    return voc_data.VOC12ClassificationDatasetMSF(list_path, voc12_root=args.voc12_root, scales=scales,
-                                                  decode_only=device_pyramid(args), raw_jpeg=device_jpeg(args), cam_dir=cam_dir)
+        return voc_data.SyntheticMSF(int(args.synthetic), scales=scales, name_list=names, decode_only=decode_only, cam_dir=cam_dir,
+                                     cam_field=cam_field)
+    return voc_data.VOC12ClassificationDatasetMSF(list_path, voc12_root=args.voc12_root, scales=scales, decode_only=decode_only,
+                                                  raw_jpeg=device_jpeg(args) and not raw_images, cam_dir=cam_dir, cam_field=cam_field)
 
 
 _jpeg_decoders = {}
@@ -246,9 +250,11 @@ class StepContext:
     def __init__(self, model, args, device, scales):
         from ..pipeline import PseudoLabelPipeline
         self.model, self.args, self.device, self.scales = model, args, device, tuple(scales)
-        is_cam = hasattr(model, "classifier")
-        self.pipe = PseudoLabelPipeline(model if is_cam else None, None if is_cam else model, device, self.scales,
-                                        beta=float(getattr(args, "beta", 10)), exp_times=int(getattr(args, "exp_times", 8)))
+        self.pipe = None
+        if model is not None:      # cam_to_ir_label has no network
+            is_cam = hasattr(model, "classifier")
+            self.pipe = PseudoLabelPipeline(model if is_cam else None, None if is_cam else model, device, self.scales,
+                                            beta=float(getattr(args, "beta", 10)), exp_times=int(getattr(args, "exp_times", 8)))
         self.writer = Writer(device)
         self._pinned = {}
         self._jpeg = None
@@ -324,23 +330,25 @@ def threaded_loader(shard, n_threads, prefetch):
 
 def work_loop(process_id, model, dataset, args, per_image, per_batch=None):
     """One GPU's share: the reference's `_work(process_id, model, dataset, args)` signature and loop order
-    (step/make_cam.py:16-59), with the per-image / per-batch body supplied by the step."""
+    (step/make_cam.py:16-59), with the per-image / per-batch body supplied by the step.  model None: a step without a network
+    (cam_to_ir_label), whose items are the decoded images themselves."""
     shard = dataset[process_id]
     n_gpus = max(torch.cuda.device_count(), 1)
     scales = getattr(getattr(shard, "dataset", shard), "scales", (1.0,))
     bsz = step_batch(args)
     workers = args.num_workers // n_gpus
-    batched = not (per_batch is None or bsz == 1 or not device_pyramid(args))
+    batched = not (per_batch is None or bsz == 1 or not (device_pyramid(args) or model is None))
     if batched:     # items travel in chunks (collate_chunk); the workers keep about two buckets' worth of them in flight
         depth = {"prefetch_factor": max(2, -(-2 * bsz // (workers * LOADER_CHUNK)))} if workers > 0 else {}
         loader = DataLoader(shard, shuffle=False, batch_size=LOADER_CHUNK, num_workers=workers, pin_memory=False, collate_fn=collate_chunk, **depth)
     else:
         loader = DataLoader(shard, shuffle=False, num_workers=workers, pin_memory=False, collate_fn=collate_one)
     with torch.no_grad(), torch.cuda.device(process_id):
-        model.cuda()
+        if model is not None:
+            model.cuda()
         if not batched:
             for it, pack in enumerate(loader):
-                per_image(model, attach_pyramid(pack, scales), args)
+                per_image(model, attach_pyramid(pack, scales) if model is not None else pack, args)
                 progress(process_id, n_gpus, it, len(shard))
             return
         ctx = StepContext(model, args, torch.device("cuda", process_id), scales)
@@ -384,16 +392,23 @@ def work_loop(process_id, model, dataset, args, per_image, per_batch=None):
                   (process_id, ", ".join("%s %.2f" % kv for kv in sorted(ctx.phase_seconds.items(), key=lambda kv: -kv[1]))), file=sys.stderr, flush=True)
 
 
-def run_step(args, work, module_name, class_name, weights_path, strict, list_path, scales, opening="[ ", cam_dir=None):
+def run_step(args, work, module_name, class_name, weights_path, strict, list_path, scales, opening="[ ", cam_dir=None, cam_field="cam"):
     """The reference's `run(args)` (e.g. step/make_cam.py:62-77): model class resolved by name, checkpoint loaded,
-    stride partition (misc/torchutils.py:66-68), one process per GPU (a single GPU runs in-process)."""
-    model = getattr(importlib.import_module(module_name), class_name)()
-    model.load_state_dict(torch.load(weights_path), strict=strict)
-    model.eval()
+    stride partition (misc/torchutils.py:66-68), one process per GPU (a single GPU runs in-process).  module_name None: a step
+    without a network (step/cam_to_ir_label.py:44-51); `work` then gets model None and the decoded uint8 images."""
+    model = None
+    if module_name is not None:
+        model = getattr(importlib.import_module(module_name), class_name)()
+        model.load_state_dict(torch.load(weights_path), strict=strict)
+        model.eval()
     n_gpus = torch.cuda.device_count()
     if n_gpus <= 0:
         raise RuntimeError("irn_b200 steps need at least one CUDA device (there is no CPU fallback)")
-    shards = torchutils.split_dataset(make_dataset(args, list_path, scales, cam_dir), n_gpus)
+    if model is None:
+        dataset = make_dataset(args, list_path, scales, cam_dir, cam_field, raw_images=True)
+    else:
+        dataset = make_dataset(args, list_path, scales, cam_dir)
+    shards = torchutils.split_dataset(dataset, n_gpus)
     print(opening, end="")
     if n_gpus == 1:
         work(0, model, shards, args)
@@ -403,13 +418,14 @@ def run_step(args, work, module_name, class_name, weights_path, strict, list_pat
     torch.cuda.empty_cache()
 
 
-def load_cam_dicts(ctx, packs, names, cam_out_dir):
+def load_cam_dicts(ctx, packs, names, cam_out_dir, field="cam"):
     """The stored CAMs of make_cam for a batch (np.load(...).item(), step/make_sem_seg_labels.py:34): what the loader workers
-    attached to the items (voc12.dataloader.attach_cam), else read here on the file pool.  Returns (keys list, cam list)."""
+    attached to the items (voc12.dataloader.attach_cam), else read here on the file pool.  Returns (keys list, list of the
+    dicts' `field` maps)."""
     if "cam" in packs[0]:
         return [p["cam_keys"][0].numpy() for p in packs], [p["cam"][0] for p in packs]
     stored = ctx.writer.map(lambda n: np.load(os.path.join(cam_out_dir, n + ".npy"), allow_pickle=True).item(), names)
-    return [np.asarray(s["keys"]) for s in stored], [s["cam"] for s in stored]
+    return [np.asarray(s["keys"]) for s in stored], [s[field] for s in stored]
 
 
 def to_device_list(ctx, tensors):

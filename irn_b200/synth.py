@@ -136,3 +136,23 @@ def normalize_image(img_u8):
     for c in range(3):
         out[..., c] = (a[..., c] / 255. - mean[c]) / std[c]
     return np.ascontiguousarray(out.transpose(2, 0, 1))
+
+
+def cam_planes_u8(K, H, W, seed=0):
+    """K structured CAM-like planes quantised to uint8 (a few Gaussian blobs each, peak 255): the stored CAMs of the
+    cam_to_ir_label fixtures are `u8 / 255` in float32, so the exact inputs travel as compressible bytes."""
+    rs = np.random.RandomState(seed)
+    y, x = np.mgrid[0:H, 0:W].astype(np.float64)
+    out = np.zeros((K, H, W), np.uint8)
+    for k in range(K):
+        a = np.zeros((H, W))
+        for _ in range(rs.randint(1, 4)):
+            cy, cx = rs.uniform(0, H), rs.uniform(0, W)
+            sy, sx = rs.uniform(0.08, 0.3) * H, rs.uniform(0.08, 0.3) * W
+            a += rs.uniform(0.3, 1.0) * np.exp(-0.5 * (((y - cy) / sy) ** 2 + ((x - cx) / sx) ** 2))
+        out[k] = np.round(255 * a / a.max()).astype(np.uint8)
+    return out
+
+
+def u8_to_cam(u8):
+    return np.asarray(u8).astype(np.float32) / np.float32(255)

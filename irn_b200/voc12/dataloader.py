@@ -71,7 +71,8 @@ class VOC12ClassificationDatasetMSF(Dataset):
     "size": (H, W), "label": FloatTensor[20]}."""
 
     def __init__(self, img_name_list_path, voc12_root, img_normal=TorchvisionNormalize(), scales=(1.0,),
-                 cls_labels_path="voc12/cls_labels.npy", decode_only=False, raw_jpeg=False, cam_dir=None):
+                 cls_labels_path="voc12/cls_labels.npy", decode_only=False, raw_jpeg=False, cam_dir=None, cam_field="cam"):
+        self.cam_field = cam_field          # which map of the CAM dict the worker ships (attach_cam)
         self.decode_only = decode_only      # hand over the decoded uint8 image; the pyramid is built on the device
         self.raw_jpeg = raw_jpeg            # hand over the FILE BYTES; nvJPEG decodes them on the device (irn_b200.jpeg)
         self.cam_dir = cam_dir              # label steps: the loader worker also reads the image's stored CAM dict (make_cam's .npy)
@@ -95,7 +96,7 @@ class VOC12ClassificationDatasetMSF(Dataset):
             if is_jpeg:
                 with open(path, "rb") as f:
                     data = np.frombuffer(f.read(), dtype=np.uint8).copy()
-                return attach_cam({"name": name_str, "size": (h, w), "label": torch.from_numpy(self.label_list[idx]), "jpeg": data}, self.cam_dir)
+                return attach_cam({"name": name_str, "size": (h, w), "label": torch.from_numpy(self.label_list[idx]), "jpeg": data}, self.cam_dir, self.cam_field)
             # not a 3-component JPEG (grey-scale / PNG stand-ins): decode on the host like the reference
         img = np.asarray(Image.open(get_img_path(name_str, self.voc12_root)).convert("RGB"))
         out = {"name": name_str, "size": (img.shape[0], img.shape[1]), "label": torch.from_numpy(self.label_list[idx])}
@@ -103,18 +104,19 @@ class VOC12ClassificationDatasetMSF(Dataset):
             out["img_u8"] = np.array(img)            # writable copy: torch's collate wraps it without a warning
         else:
             out["img"] = multi_scale_flip(img, self.scales, self.img_normal)
-        attach_cam(out, self.cam_dir)
+        attach_cam(out, self.cam_dir, self.cam_field)
         return out
 
 
-def attach_cam(item, cam_dir):
+def attach_cam(item, cam_dir, field="cam"):
     """The label steps read `np.load(cam_out_dir/<name>.npy).item()` per image in their main loop
     (step/make_sem_seg_labels.py:34-37); with `cam_dir` set the loader WORKER does that read, in parallel with the decode, and
-    ships what the steps use of it: `cam_keys` int64 [K] and `cam` fp32 [K,h/4,w/4] (not the full-resolution maps)."""
+    ships what the steps use of it: `cam_keys` int64 [K] and, as item["cam"], the dict's `field`: the strided `cam` fp32
+    [K,h/4,w/4] for the random-walk steps, the full-resolution `high_res` fp32 [K,H,W] for cam_to_ir_label."""
     if cam_dir:
         d = np.load(os.path.join(cam_dir, item["name"] + ".npy"), allow_pickle=True).item()
         item["cam_keys"] = torch.as_tensor(np.asarray(d["keys"]), dtype=torch.int64)
-        item["cam"] = torch.as_tensor(np.asarray(d["cam"]), dtype=torch.float32).contiguous()
+        item["cam"] = torch.as_tensor(np.asarray(d[field]), dtype=torch.float32).contiguous()
     return item
 
 
@@ -123,8 +125,8 @@ class SyntheticMSF(Dataset):
     ids are taken from an image-name list when given, else 2007_000000 + index."""
 
     def __init__(self, n_items, size=(512, 512), scales=(1.0,), name_list=None, img_normal=TorchvisionNormalize(), decode_only=False,
-                 cam_dir=None):
-        self.cam_dir = cam_dir
+                 cam_dir=None, cam_field="cam"):
+        self.cam_dir, self.cam_field = cam_dir, cam_field
         self.decode_only = decode_only       # (no module stored on the instance: shards are pickled for spawn / DataLoader workers)
         self.n, self.size, self.scales, self.img_normal = n_items, size, scales, img_normal
         self.names = None if name_list is None else load_img_name_list(name_list)[:n_items]
@@ -141,4 +143,4 @@ class SyntheticMSF(Dataset):
             out["img_u8"] = np.array(img)
         else:
             out["img"] = multi_scale_flip(img, self.scales, self.img_normal)
-        return attach_cam(out, self.cam_dir)
+        return attach_cam(out, self.cam_dir, self.cam_field)

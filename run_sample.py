@@ -3,8 +3,9 @@
 
 Every flag name and default of the reference (run_sample.py:11-72) is accepted and the output directories are the same,
 so the reference's evaluation steps (step/eval_cam.py, step/eval_sem_seg.py, step/eval_ins_seg.py) read
-``result/cam/*.npy``, ``result/sem_seg/*.png`` and ``result/ins_seg/*.npy`` unchanged.  Only the three hot-path steps
-run here (make_cam, make_ins_seg_labels, make_sem_seg_labels); training / CRF / evaluation passes are the reference's own.
+``result/cam/*.npy``, ``result/sem_seg/*.png`` and ``result/ins_seg/*.npy`` unchanged.  The four inference steps run here
+(make_cam, cam_to_ir_label -- the CRF on the GPU, writing ``result/ir_label/*.png`` --, make_ins_seg_labels, make_sem_seg_labels),
+in the reference's order; the evaluation passes run when VOC ground truth is present; the training passes are the reference's own.
 
 Differences: --cam_network / --irn_network default to the irn_b200 modules; flags the reference declares without a type
 (--beta, --exp_times, --*_bg_thres, --*_pass) are parsed; --synthetic N runs on N seeded synthetic images instead of VOC
@@ -42,7 +43,8 @@ FLAGS = [
     ("sem_seg_out_dir", "result/sem_seg", str), ("ins_seg_out_dir", "result/ins_seg", str),
 ]
 PASSES = ["train_cam", "make_cam", "eval_cam", "cam_to_ir_label", "train_irn", "make_ins_seg", "eval_ins_seg", "make_sem_seg", "eval_sem_seg"]
-HOT_STEPS = {"make_cam": "make_cam", "make_ins_seg": "make_ins_seg_labels", "make_sem_seg": "make_sem_seg_labels"}   # pass -> module
+HOT_STEPS = {"make_cam": "make_cam", "cam_to_ir_label": "cam_to_ir_label", "make_ins_seg": "make_ins_seg_labels",
+             "make_sem_seg": "make_sem_seg_labels"}   # pass -> module
 EVAL_STEPS = {"eval_cam": "eval_cam", "eval_sem_seg": "eval_sem_seg", "eval_ins_seg": "eval_ins_seg"}   # host-side evaluators (need VOC ground truth)
 
 
