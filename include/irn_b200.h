@@ -163,6 +163,27 @@ void irn_conv_destroy(irn_conv* conv);
 int irn_conv_forward(irn_conv* conv, const float* in, int B, int H, int W, const float* residual,
                      float* out, int relu, int mode, irn_stream_t stream);
 
+/* The networks' stem (conv 7x7/2 pad 3, 3 -> 64, + folded FixedBatchNorm, ReLU) as a plan of its own, run by the
+ * same code as the trunk: input layout transform, then the SIMT (mode 0), 3xTF32 (mode 1) or f16x3 (mode 2) stem.
+ *   weight_oihw HOST fp32 [64,3,7,7]; bn4 HOST fp32 [4,64] or NULL.  Free with irn_conv_destroy.
+ *   forward: x_nchw fp32 [B,3,H,W] zero-padded on the right / bottom to Hin x Win (H <= Hin, W <= Win) ->
+ *   out_nhwc [B,Ho,Wo,64], Ho = (Hin-1)/2+1, Wo = (Win-1)/2+1; workspace device, 256-byte aligned,
+ *   >= irn_stem_workspace_bytes(B, Hin, Win). */
+int irn_stem_create(const float* weight_oihw, const float* bn4, irn_conv** out);
+size_t irn_stem_workspace_bytes(int B, int Hin, int Win);
+int irn_stem_forward(irn_conv* stem, const float* x_nchw, int B, int H, int W, int Hin, int Win,
+                     float* out_nhwc, int mode, void* workspace, size_t workspace_bytes, irn_stream_t stream);
+
+/* conv3 and the projection shortcut of a ResNet-50 stage's first bottleneck as the f16x3 network runs them: one
+ * K-concatenated 1x1 conv, out = relu(bn3(conv3(t2)) + bnds(ds(x sampled at `stride`))).
+ *   w3 HOST fp32 [4 planes, planes]; wds HOST fp32 [4 planes, cin]; bn3, bnds HOST fp32 [4, 4 planes] (both required).
+ *   Fails unless planes % 64 == 0 and cin % 64 == 0.  Free with irn_conv_destroy.
+ *   forward: x NHWC fp32 [B,H,W,cin]; t2 NHWC [B,Ho,Wo,planes] and out NHWC [B,Ho,Wo,4 planes], Ho = (H-1)/stride+1. */
+int irn_shortcut_conv_create(const float* w3, const float* bn3, const float* wds, const float* bnds, int planes,
+                             int cin, int stride, irn_conv** out);
+int irn_shortcut_conv_forward(irn_conv* conv, const float* t2, const float* x, int B, int H, int W, float* out,
+                              irn_stream_t stream);
+
 /* CAM.forward over B/2 (image, horizontally flipped image) pairs.
  *   x_nchw fp32 [B,3,H,W] (device), B even -> cam fp32 [B/2,20,ceil(H/16),ceil(W/16)]:
  *   relu(classifier(trunk(x)))[2p] + relu(...)[2p+1].flip(-1)   (net/resnet50_cam.py:65-68) */

@@ -41,6 +41,12 @@ SIGNATURES = {
     "irn_conv_create": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
     "irn_conv_destroy": (None, [c_void_p]),
     "irn_conv_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "irn_stem_create": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_void_p)]),
+    "irn_stem_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "irn_stem_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_size_t,
+                                 c_void_p]),
+    "irn_shortcut_conv_create": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
+    "irn_shortcut_conv_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "irn_cam_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "irn_cam_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "irn_edge_displacement_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),

@@ -221,11 +221,11 @@ static int read_vec(irn_net* net, Reader& rd, size_t n, float** out) {
     return upload(net, std::vector<float>(p, p + n), out);
 }
 
-static int read_trunk(irn_net* net, Reader& rd) {
-    int rc = read_conv(net, rd, net->stem, 3, 64, 7, 2, 3, true);
-    if (rc) return rc;
+// Repacks the folded 7x7/s2 stem (read_conv'd into `c`) for the tensor-core kernels over the zero-haloed NHWC4 input: the 3xTF32
+// planes of `c` and the f16x3 conv `f`
+static int build_stem(irn_net* net, Conv& c, Conv& f) {
+    int rc;
     {   // tensor-core stem: K = 7 rows x (8 taps x 4 channels) = 224, tap 7 and channel 3 carry zero weights
-        Conv& c = net->stem;
         std::vector<float> host((size_t)49 * 3 * 64);
         IRN_CUDA(cudaMemcpy(host.data(), c.wt, host.size() * sizeof(float), cudaMemcpyDeviceToHost));
         const size_t K = 224;
@@ -253,7 +253,6 @@ static int read_trunk(irn_net* net, Reader& rd) {
         if ((rc = make_tensor_map(&c.map_blo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c.w_lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
         c.stem_tc = true;
         // f16x3 stem: the same rows, K = 8 filter rows x 32 (row 7 zero) = 256 = four 64-wide k-blocks
-        Conv& f = net->stem_f16;
         f.cin = 256; f.cout = 64; f.k = 1; f.stride = 1; f.pad = 0;
         std::vector<float> wt((size_t)256 * 64, 0.f);
         for (int o = 0; o < 64; ++o)
@@ -264,6 +263,32 @@ static int read_trunk(irn_net* net, Reader& rd) {
         f.bias = c.bias;
         if ((rc = make_bf16_weights(net, f, wt))) return rc;
     }
+    return kOk;
+}
+
+// f16x3 mode: conv3 and the projection shortcut of a first block (both read_conv'd with BN, host copies still present) as one
+// K-concatenated 1x1 conv; blk.has_c3ds says whether it was eligible
+static int build_c3ds(irn_net* net, Block& blk, int cin, int planes) {
+    blk.has_c3ds = false;
+    if (planes % kBfBK != 0 || cin % kBfBK != 0) return kOk;
+    Conv& f = blk.c3ds;
+    const int cout = planes * 4, K3 = planes, Kd = cin;
+    f.cin = K3 + Kd; f.cout = cout; f.k = 1; f.stride = 1; f.pad = 0;
+    std::vector<float> wt((size_t)(K3 + Kd) * cout), bias(cout);
+    std::copy(blk.c3.host_wt.begin(), blk.c3.host_wt.end(), wt.begin());
+    std::copy(blk.ds.host_wt.begin(), blk.ds.host_wt.end(), wt.begin() + (size_t)K3 * cout);
+    for (int o = 0; o < cout; ++o) bias[o] = blk.c3.host_bias[o] + blk.ds.host_bias[o];
+    int rc;
+    if ((rc = upload(net, bias, &f.bias))) return rc;
+    if ((rc = make_bf16_weights(net, f, wt))) return rc;
+    blk.has_c3ds = f.bf_ok;
+    return kOk;
+}
+
+static int read_trunk(irn_net* net, Reader& rd) {
+    int rc = read_conv(net, rd, net->stem, 3, 64, 7, 2, 3, true);
+    if (rc) return rc;
+    if ((rc = build_stem(net, net->stem, net->stem_f16))) return rc;
     int cin = 64;
     for (int l = 0; l < 4; ++l) {
         net->blocks[l].resize(kBlocks[l]);
@@ -275,18 +300,7 @@ static int read_trunk(irn_net* net, Reader& rd) {
             if ((rc = read_conv(net, rd, blk.c3, planes, planes * 4, 1, 1, 0, true))) return rc;
             blk.has_ds = b == 0;
             if (blk.has_ds && (rc = read_conv(net, rd, blk.ds, cin, planes * 4, 1, stride, 0, true))) return rc;
-            if (blk.has_ds && planes % kBfBK == 0 && cin % kBfBK == 0) {
-                Conv& f = blk.c3ds;
-                const int cout = planes * 4, K3 = planes, Kd = cin;
-                f.cin = K3 + Kd; f.cout = cout; f.k = 1; f.stride = 1; f.pad = 0;
-                std::vector<float> wt((size_t)(K3 + Kd) * cout), bias(cout);
-                std::copy(blk.c3.host_wt.begin(), blk.c3.host_wt.end(), wt.begin());
-                std::copy(blk.ds.host_wt.begin(), blk.ds.host_wt.end(), wt.begin() + (size_t)K3 * cout);
-                for (int o = 0; o < cout; ++o) bias[o] = blk.c3.host_bias[o] + blk.ds.host_bias[o];
-                if ((rc = upload(net, bias, &f.bias))) return rc;
-                if ((rc = make_bf16_weights(net, f, wt))) return rc;
-                blk.has_c3ds = f.bf_ok;
-            }
+            if (blk.has_ds && (rc = build_c3ds(net, blk, cin, planes))) return rc;
             cin = planes * 4;
         }
     }
@@ -496,14 +510,48 @@ static TrunkShapes trunk_shapes(int B, int H, int W) {
     return s;
 }
 
+// conv3 + projection shortcut in one reduction (Block::c3ds): out = relu([W3 | Wds] . [t2 ; x sampled at the block's stride] + b3 + bds),
+// x NHWC on the block's input grid h x w, t2 and out on its output grid ho x wo
+static int run_c3ds(const Block& blk, const float* t2, const float* x, int B, int h, int w, int ho, int wo, float* out, cudaStream_t st) {
+    F16Second sec;
+    sec.in = x; sec.H = h; sec.W = w; sec.cin = blk.ds.cin; sec.stride = blk.ds.stride;
+    return run_conv_f16(blk.c3ds, t2, B, ho, wo, ho, wo, nullptr, out, true, st, &sec);
+}
+
+static bool stem_on_tensor_cores(const irn_net* net) { return net->conv_mode >= 1 && net->stem.stem_tc; }
+
+// floats of run_stem's input buffer x_in: the zero-haloed NHWC4 layout for the tensor-core stems, plain NHWC otherwise
+static size_t stem_input_floats(const irn_net* net, int B, int Hin, int Win) {
+    return stem_on_tensor_cores(net) ? (size_t)B * (Hin + 6) * (Win + 8) * 4 : (size_t)B * Hin * Win * 3;
+}
+
+// The stem of the trunk: x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win is laid out in x_in (stem_input_floats), then
+// conv 7x7/s2 + bias + ReLU -> out NHWC [B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), 64]
+static int run_stem(const irn_net* net, const float* x_nchw, int B, int H, int W, int Hin, int Win, float* x_in, float* out,
+                    cudaStream_t st) {
+    int rc;
+    if (stem_on_tensor_cores(net)) {
+        const size_t total = (size_t)B * (Hin + 6) * (Win + 8);
+        nchw_to_nhwc4_halo_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, (float4*)x_in, B, H, W, Hin + 6, Win + 8);
+        IRN_LAUNCH_CHECK("nchw_to_nhwc4_halo_kernel");
+        static const int stem_f16 = getenv("IRN_F16_STEM") ? atoi(getenv("IRN_F16_STEM")) : 1;
+        if (net->conv_mode == 2 && net->stem_f16.bf_ok && stem_f16) return launch_f16_stem(net->stem_f16, x_in, B, Hin, Win, out, st);
+        return launch_tf32_stem(net->stem, x_in, B, Hin, Win, out, st);
+    }
+    const size_t total = (size_t)B * Hin * Win * 3;
+    nchw_to_nhwc_pad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, x_in, B, 3, H, W, Hin, Win);
+    IRN_LAUNCH_CHECK("nchw_to_nhwc_pad_kernel");
+    if ((rc = run_conv(net, net->stem, x_in, B, Hin, Win, nullptr, out, true, st, nullptr, nullptr))) return rc;
+    return kOk;
+}
+
 // Runs input layout transform + stem + maxpool + layer1..4 on x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win.
 // feats[0] = after maxpool (x1 of IRNet), feats[1..4] = layer outputs.  When `keep` is set every feats[i] lives in
 // its own arena buffer (IRNet taps them); otherwise buffers rotate.
 static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int W, int Hin, int Win, Arena& ar, bool keep,
                      const float* feats[5], TrunkShapes& sh, cudaStream_t st) {
     sh = trunk_shapes(B, Hin, Win);
-    const bool stem_tc = net->conv_mode >= 1 && net->stem.stem_tc;
-    float* x_in = stem_tc ? ar.take((size_t)B * (Hin + 6) * (Win + 8) * 4) : ar.take((size_t)B * Hin * Win * 3);
+    float* x_in = ar.take(stem_input_floats(net, B, Hin, Win));
     float* stem_out = ar.take((size_t)B * sh.H1 * sh.W1 * 64);
     float* pool_out = ar.take((size_t)B * sh.H2 * sh.W2 * 64);
     float* t1 = ar.take(sh.max_act);
@@ -512,20 +560,7 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
     float* ping[2] = {ar.take(sh.max_act), ar.take(sh.max_act)};
     if (!ar.ok) return fail(kWorkspace, "network workspace too small");
     int rc;
-    if (stem_tc) {
-        const size_t total = (size_t)B * (Hin + 6) * (Win + 8);
-        nchw_to_nhwc4_halo_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, (float4*)x_in, B, H, W, Hin + 6, Win + 8);
-        IRN_LAUNCH_CHECK("nchw_to_nhwc4_halo_kernel");
-        static const int stem_f16 = getenv("IRN_F16_STEM") ? atoi(getenv("IRN_F16_STEM")) : 1;
-        if (net->conv_mode == 2 && net->stem_f16.bf_ok && stem_f16) {
-            if ((rc = launch_f16_stem(net->stem_f16, x_in, B, Hin, Win, stem_out, st))) return rc;
-        } else if ((rc = launch_tf32_stem(net->stem, x_in, B, Hin, Win, stem_out, st))) return rc;
-    } else {
-        const size_t total = (size_t)B * Hin * Win * 3;
-        nchw_to_nhwc_pad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, x_in, B, 3, H, W, Hin, Win);
-        IRN_LAUNCH_CHECK("nchw_to_nhwc_pad_kernel");
-        if ((rc = run_conv(net, net->stem, x_in, B, Hin, Win, nullptr, stem_out, true, st, nullptr, nullptr))) return rc;
-    }
+    if ((rc = run_stem(net, x_nchw, B, H, W, Hin, Win, x_in, stem_out, st))) return rc;
     {
         const size_t total = (size_t)B * sh.H2 * sh.W2 * 16;
         maxpool3s2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(stem_out, pool_out, B, sh.H1, sh.W1, 64, sh.H2, sh.W2);
@@ -556,10 +591,8 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
                 out = ping[flip];
                 flip ^= 1;
             }
-            if (fused) {   // conv3 + projection shortcut in one reduction: [t2 ; x sampled at the block's stride]
-                F16Second sec;
-                sec.in = x; sec.H = h; sec.W = w; sec.cin = blk.ds.cin; sec.stride = blk.ds.stride;
-                if ((rc = run_conv_f16(blk.c3ds, t2, B, ho, wo, ho, wo, nullptr, out, true, st, &sec))) return rc;
+            if (fused) {
+                if ((rc = run_c3ds(blk, t2, x, B, h, w, ho, wo, out, st))) return rc;
             } else if ((rc = run_conv(net, blk.c3, t2, B, ho, wo, res, out, true, st, nullptr, nullptr))) return rc;   // out += residual; relu (net/resnet50.py:51-52)
             x = out;
             h = ho;
@@ -610,6 +643,78 @@ extern "C" void irn_conv_destroy(irn_conv* c) {
     if (!c) return;
     for (void* p : c->holder.allocs) cudaFree(p);
     delete c;
+}
+
+// The network's stem as a plan of its own, built and run by the same code as the trunk's (build_stem, run_stem)
+extern "C" int irn_stem_create(const float* weight_oihw, const float* bn4, irn_conv** out) {
+    if (!weight_oihw || !out) return fail(kBadArg, "irn_stem_create: bad argument");
+    std::vector<float> blob(weight_oihw, weight_oihw + (size_t)64 * 3 * 7 * 7);
+    if (bn4) blob.insert(blob.end(), bn4, bn4 + 4 * 64);
+    irn_conv* c = new irn_conv();
+    Reader rd{blob.data(), blob.size()};
+    int rc = read_conv(&c->holder, rd, c->holder.stem, 3, 64, 7, 2, 3, bn4 != nullptr);
+    if (!rc) rc = build_stem(&c->holder, c->holder.stem, c->holder.stem_f16);
+    if (rc) {
+        irn_conv_destroy(c);
+        return rc;
+    }
+    *out = c;
+    return kOk;
+}
+
+extern "C" size_t irn_stem_workspace_bytes(int B, int Hin, int Win) {
+    if (B <= 0 || Hin <= 0 || Win <= 0) return 0;
+    return (size_t)B * (Hin + 6) * (Win + 8) * 4 * sizeof(float);   // the larger of the two stem_input_floats layouts
+}
+
+extern "C" int irn_stem_forward(irn_conv* c, const float* x_nchw, int B, int H, int W, int Hin, int Win, float* out_nhwc, int mode,
+                                void* workspace, size_t workspace_bytes, irn_stream_t stream) {
+    launch_counter() = 0;
+    if (!c || !c->holder.stem.stem_tc || !x_nchw || !out_nhwc || !workspace) return fail(kBadArg, "irn_stem_forward: bad argument");
+    if (B <= 0 || H <= 0 || W <= 0 || H > Hin || W > Win)
+        return fail(kBadArg, "irn_stem_forward: need B > 0 and 0 < H <= Hin, 0 < W <= Win; got B=%d H=%d W=%d Hin=%d Win=%d", B, H, W, Hin, Win);
+    if (mode < 0 || mode > 2) return fail(kBadArg, "irn_stem_forward: mode must be 0, 1 or 2");
+    if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "irn_stem_forward: workspace must be 256-byte aligned");
+    if (workspace_bytes < irn_stem_workspace_bytes(B, Hin, Win)) return fail(kWorkspace, "irn_stem_forward: workspace too small");
+    c->holder.conv_mode = mode;
+    return run_stem(&c->holder, x_nchw, B, H, W, Hin, Win, (float*)workspace, out_nhwc, (cudaStream_t)stream);
+}
+
+// conv3 + projection shortcut of a first bottleneck block as the f16x3 network runs them: one K-concatenated 1x1 conv (build_c3ds)
+extern "C" int irn_shortcut_conv_create(const float* w3, const float* bn3, const float* wds, const float* bnds, int planes, int cin,
+                                        int stride, irn_conv** out) {
+    if (!w3 || !bn3 || !wds || !bnds || !out || planes <= 0 || cin <= 0 || !(stride == 1 || stride == 2))
+        return fail(kBadArg, "irn_shortcut_conv_create: bad argument");
+    if (planes % kBfBK != 0 || cin % kBfBK != 0)
+        return fail(kUnsupported, "irn_shortcut_conv_create: the fused conv needs planes %% %d == 0 and cin %% %d == 0 (got %d, %d)", kBfBK,
+                    kBfBK, planes, cin);
+    const int cout = planes * 4;
+    std::vector<float> b3(w3, w3 + (size_t)cout * planes), bd(wds, wds + (size_t)cout * cin);
+    b3.insert(b3.end(), bn3, bn3 + 4 * (size_t)cout);
+    bd.insert(bd.end(), bnds, bnds + 4 * (size_t)cout);
+    irn_conv* c = new irn_conv();
+    Block& blk = c->holder.blocks[0].emplace_back();
+    Reader r3{b3.data(), b3.size()}, rd{bd.data(), bd.size()};
+    int rc = read_conv(&c->holder, r3, blk.c3, planes, cout, 1, 1, 0, true);
+    if (!rc) rc = read_conv(&c->holder, rd, blk.ds, cin, cout, 1, stride, 0, true);
+    blk.has_ds = true;
+    if (!rc) rc = build_c3ds(&c->holder, blk, cin, planes);
+    if (!rc && !blk.has_c3ds) rc = fail(kUnsupported, "irn_shortcut_conv_create: the fused conv is not eligible for the f16x3 kernel");
+    if (rc) {
+        irn_conv_destroy(c);
+        return rc;
+    }
+    *out = c;
+    return kOk;
+}
+
+// relu(conv3(t2) + shortcut(x)): x NHWC [B,H,W,cin], t2 and out NHWC on the strided grid [B,Ho,Wo,planes | 4 planes]
+extern "C" int irn_shortcut_conv_forward(irn_conv* c, const float* t2, const float* x, int B, int H, int W, float* out, irn_stream_t stream) {
+    launch_counter() = 0;
+    if (!c || c->holder.blocks[0].size() != 1 || !t2 || !x || !out || B <= 0 || H <= 0 || W <= 0)
+        return fail(kBadArg, "irn_shortcut_conv_forward: bad argument");
+    const Block& blk = c->holder.blocks[0][0];
+    return run_c3ds(blk, t2, x, B, H, W, conv_out(H, 1, blk.ds.stride, 0), conv_out(W, 1, blk.ds.stride, 0), out, (cudaStream_t)stream);
 }
 
 // in NHWC fp32 [B,H,W,cin] -> out NHWC [B,Ho,Wo,cout]; residual NHWC like out or NULL; mode as irn_net_set_conv_mode

@@ -1,6 +1,7 @@
 """Small-shape tour of every hand-written kernel family, meant to run under compute-sanitizer (memcheck / racecheck /
 initcheck): fused cluster walk at every cluster size 1..16, the per-step walk, the wgmma convolution kernels (3xTF32 and
-bf16x3, every N tile), labels, CAM merge, instance kernels, input pyramids.
+f16x3, every N tile, the tensor-core stems, the fused conv3 + projection shortcut), labels, CAM merge, instance kernels, input
+pyramids.
     compute-sanitizer --tool memcheck python tools/sanitize_small.py"""
 import os
 import sys
@@ -10,7 +11,7 @@ import numpy as np
 import torch
 
 from irn_b200 import cam_ops, indexing, instance, preprocess, synth
-from irn_b200.ops import Conv2d
+from irn_b200.ops import Conv2d, ShortcutConv, Stem
 
 dev = torch.device("cuda:0")
 t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
@@ -37,6 +38,14 @@ for cin, cout, k, s, H, W, res in [(64, 64, 3, 1, 20, 24, False), (64, 256, 1, 1
         conv(x, r, relu=True, mode=mode)
     torch.cuda.synchronize()
     print("conv", cin, cout, k, s, "ok", flush=True)
+bn = lambda n: [np.ones(n, np.float32), np.zeros(n, np.float32), np.zeros(n, np.float32), np.ones(n, np.float32)]
+stem = Stem((torch.randn(64, 3, 7, 7) * 0.05).numpy(), bn(64))
+for mode in (1, 2):
+    stem(torch.randn(2, 3, 30, 41).to(dev), 48, 48, mode=mode)   # crop padding: H, W < Hin, Win
+sc = ShortcutConv((torch.randn(512, 128) * 0.05).numpy(), bn(512), (torch.randn(512, 256) * 0.05).numpy(), bn(512), 2)
+sc(torch.randn(2, 7, 9, 128).to(dev), torch.randn(2, 13, 17, 256).to(dev))
+torch.cuda.synchronize()
+print("stem, fused shortcut ok", flush=True)
 
 # labels, merge, instance kernels, pyramids
 rw = torch.rand(3, 20, 24).to(dev)
