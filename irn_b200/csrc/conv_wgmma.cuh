@@ -54,7 +54,7 @@ struct TcArgs {
     int kb_split = 1 << 30;          // f16x3 only: k-blocks [kb_split, KB) read input `a2` (pixel stride `stride2`): the projection
     int stride2 = 1;                 // shortcut of a bottleneck fused into conv3's reduction (nets.cu, Block::c3ds)
     const float* oscale = nullptr;   // f16x3 only: per-output-channel factor undoing the weights' power-of-two pre-scale
-    int stem = 0;                    // 1: 7x7/s2 stem over the zero-haloed NHWC4 input, k-blocks = filter rows (nets.cu, launch_*_stem)
+    int stem = 0;                    // 1: 7x7/s2 stem over the zero-haloed NHWC4 input, k-blocks = filter rows (nets.cu, run_stem)
 };
 
 template <bool F16, int BN>

@@ -4,13 +4,12 @@
 // (CAM.forward), net/resnet50_irn.py:23-133,216-234 (heads, MeanShift, EdgeDisplacement.forward).
 //
 // The plan owns the repacked weights on the device: FixedBatchNorm folded into (weight, bias), weights
-// transposed to [kh*kw*Cin][Cout] for the SIMT kernel.  Activations are NHWC fp32 in a caller-provided
-// workspace.  The host walks the fixed topology and enqueues kernels on the caller's stream; nothing
-// synchronises.
+// transposed to [kh*kw*Cin][Cout] for the SIMT kernel and split for the tensor-core kernel (SplitWeights).  Activations
+// are NHWC fp32 in a caller-provided workspace.  The host walks the fixed topology and enqueues kernels on the caller's
+// stream; nothing synchronises.
 #include <cuda_fp16.h>
 
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -20,24 +19,32 @@
 
 namespace irn {
 
+// Device allocations of a plan, freed with it
+struct DeviceAllocs {
+    std::vector<void*> ptrs;
+    DeviceAllocs() = default;
+    DeviceAllocs(const DeviceAllocs&) = delete;
+    DeviceAllocs& operator=(const DeviceAllocs&) = delete;
+    ~DeviceAllocs() {
+        for (void* p : ptrs) cudaFree(p);
+    }
+};
+
+// Weights [cout][K] (K-major) split into hi / lo planes for the tensor-core kernel in one of its two arithmetics (pack_split):
+// 3xTF32 fp32 planes, or f16x3 fp16 planes of the weights pre-scaled per output channel by a power of two
+struct SplitWeights {
+    bool ok = false;                    // packed: the conv is eligible for this arithmetic
+    const void* hi = nullptr;           // device [cout][K]
+    const void* lo = nullptr;
+    CUtensorMap map_hi[2], map_lo[2];   // boxes {one k-block, 64 | 128 rows}; [1] only when cout % 128 == 0
+    float* oscale = nullptr;            // f16x3: [cout], the inverse pre-scale applied in the epilogue
+};
+
 struct Conv {
     int cin = 0, cout = 0, k = 1, stride = 1, pad = 0;
     float* wt = nullptr;     // device [k*k*cin][cout]   (SIMT kernel)
     float* bias = nullptr;   // device [cout] or null
-    // tensor-core path: weights [cout][k*k*cin] split into tf32 hi / lo parts
-    float* w_hi = nullptr;
-    float* w_lo = nullptr;
-    int bn = 0;              // N tile (64 or 128); 0 = not eligible
-    CUtensorMap map_bhi, map_blo;        // box {32, bn}
-    // f16x3 path (conv_wgmma.cuh): weights [cout][k*k*cin], pre-scaled per output channel by a power of two and split into fp16
-    // hi / lo parts, boxes {64 k, 64 | 128 rows}; oscale[cout] = the inverse scale applied in the epilogue
-    uint16_t* wb_hi = nullptr;
-    uint16_t* wb_lo = nullptr;
-    float* oscale = nullptr;
-    bool bf_ok = false;
-    CUtensorMap map_bf_hi[2], map_bf_lo[2];   // N tile 64, 128 (the latter only when cout allows)
-    std::vector<float> host_wt, host_bias;   // folded fp32 weights [K][cout] / bias, kept on the host until the plan is complete
-    bool stem_tc = false;    // 7x7/s2 stem repacked as 7 k-blocks of (8 taps x 4 channels) over a zero-haloed NHWC4 input
+    SplitWeights tf32, f16;  // the stem's are repacked over its zero-haloed NHWC4 input (build_stem)
 };
 
 struct Head {            // conv1x1 (no bias) -> GroupNorm(groups) -> [upsample] -> ReLU
@@ -62,7 +69,6 @@ struct irn_net {
     int kind = 0;   // 0 = CAM, 1 = IRN (EdgeDisplacement)
     int conv_mode = 2;   // 0 = SIMT exact-fp32 convolutions only, 1 = wgmma 3xTF32 where eligible, 2 = wgmma f16x3 (default; 3xTF32 / SIMT for the layers it cannot take)
     irn::Conv stem;
-    irn::Conv stem_f16;            // the stem repacked for the f16x3 kernel (K = 256 over the NHWC4 halo layout)
     std::vector<irn::Block> blocks[4];
     // CAM
     float* classifier = nullptr;   // [20][2048] (SIMT head kernel)
@@ -73,7 +79,7 @@ struct irn_net {
     float* edge6_b = nullptr;      // [1]
     float* dp7_w = nullptr;        // [2][256]
     float* mean_shift = nullptr;   // [2]
-    std::vector<void*> allocs;
+    irn::DeviceAllocs mem;
 };
 
 namespace irn {
@@ -98,20 +104,95 @@ struct Reader {
     }
 };
 
-static int upload(irn_net* net, const std::vector<float>& h, float** out) {
+template <class T>
+static int upload(DeviceAllocs& mem, const std::vector<T>& h, T** out) {
     void* d = nullptr;
-    IRN_CUDA(cudaMalloc(&d, h.size() * sizeof(float)));
-    net->allocs.push_back(d);
-    IRN_CUDA(cudaMemcpy(d, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice));
-    *out = (float*)d;
+    IRN_CUDA(cudaMalloc(&d, h.size() * sizeof(T)));
+    mem.ptrs.push_back(d);
+    IRN_CUDA(cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
+    *out = (T*)d;
     return kOk;
 }
 
-static int make_bf16_weights(irn_net* net, Conv& c, const std::vector<float>& wt);
+// The tensor-core kernel takes a conv whose Cin is a multiple of the arithmetic's k-block `bk` (3xTF32 kTcBK, f16x3 kBfBK), whose
+// Cout is a multiple of the 64-wide N tile, with k 1 or 3 and stride 1 or 2
+static bool split_eligible(int cin, int cout, int k, int stride, int bk) {
+    return cin % bk == 0 && cout % 64 == 0 && (k == 1 || k == 3) && (stride == 1 || stride == 2);
+}
 
-// Reads conv weight [cout][cin][k][k] (+ optional BN gamma, beta, mean, var) and uploads the folded,
-// transposed tensors.  Fold: y = (conv - mean) / sqrt(var + 1e-5) * gamma + beta  (net/resnet50.py:11-14).
-static int read_conv(irn_net* net, Reader& rd, Conv& c, int cin, int cout, int k, int stride, int pad, bool bn) {
+// Splits folded fp32 weights wt [K][cout] into the hi / lo planes [cout][K] of one tensor-core arithmetic, uploads them and encodes
+// their tensor maps.
+//   3xTF32  hi = w rounded to nearest (ties away) to 10 explicit mantissa bits, like cvt.rna.tf32.f32; lo = w - hi.
+//   f16x3   every output channel is first scaled by a power of two so that max |w| lies in [1,2): the lo parts stay clear of fp16's
+//           subnormal range whatever FixedBatchNorm's gamma / sqrt(var) did to the channel, and the epilogue undoes the scale
+//           exactly (oscale).  hi = fp16(v), lo = fp16(v - hi), both rounded to nearest.
+static int pack_split(DeviceAllocs& mem, bool f16, const float* wt, size_t K, int cout, SplitWeights& s) {
+    const size_t n = (size_t)cout * K;
+    int rc;
+    if (f16) {
+        std::vector<uint16_t> hi(n), lo(n);
+        std::vector<float> inv(cout, 1.0f);
+        for (int o = 0; o < cout; ++o) {
+            float mx = 0.f;
+            for (size_t kk = 0; kk < K; ++kk) mx = std::max(mx, std::fabs(wt[kk * cout + o]));
+            int e = 1;
+            if (mx > 0.f && std::isfinite(mx)) std::frexp(mx, &e);          // mx = m * 2^e, m in [0.5, 1)
+            const int sh = 1 - e;                                           // w * 2^sh has its maximum in [1, 2)
+            inv[o] = std::ldexp(1.0f, -sh);
+            for (size_t kk = 0; kk < K; ++kk) {
+                const float v = std::ldexp(wt[kk * cout + o], sh);
+                const __half h = __float2half_rn(v);
+                const __half l = __float2half_rn(v - __half2float(h));
+                hi[(size_t)o * K + kk] = __half_as_ushort(h);
+                lo[(size_t)o * K + kk] = __half_as_ushort(l);
+            }
+        }
+        uint16_t *dhi, *dlo;
+        if ((rc = upload(mem, inv, &s.oscale)) || (rc = upload(mem, hi, &dhi)) || (rc = upload(mem, lo, &dlo))) return rc;
+        s.hi = dhi;
+        s.lo = dlo;
+    } else {
+        std::vector<float> hi(n), lo(n);
+        for (int o = 0; o < cout; ++o)
+            for (size_t kk = 0; kk < K; ++kk) {
+                const float v = wt[kk * cout + o];
+                uint32_t u;
+                std::memcpy(&u, &v, 4);
+                uint32_t h = (u + 0x1000u) & 0xFFFFE000u;
+                float hf;
+                std::memcpy(&hf, &h, 4);
+                if (!std::isfinite(hf)) hf = v;
+                hi[(size_t)o * K + kk] = hf;
+                lo[(size_t)o * K + kk] = v - hf;
+            }
+        float *dhi, *dlo;
+        if ((rc = upload(mem, hi, &dhi)) || (rc = upload(mem, lo, &dlo))) return rc;
+        s.hi = dhi;
+        s.lo = dlo;
+    }
+    const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)cout};
+    const uint64_t strides[1] = {(uint64_t)K * (f16 ? sizeof(uint16_t) : sizeof(float))};
+    for (int i = 0; i < 2; ++i) {
+        const uint32_t rows = 64u << i;
+        if (cout % rows != 0) continue;
+        const uint32_t box[2] = {(uint32_t)(f16 ? kBfBK : kTcBK), rows};
+        if ((rc = make_tensor_map(&s.map_hi[i], dt, 2, s.hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+        if ((rc = make_tensor_map(&s.map_lo[i], dt, 2, s.lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    }
+    s.ok = true;
+    return kOk;
+}
+
+struct HostWeights {   // folded fp32 weights [K][cout] and bias [cout] (empty without BN)
+    std::vector<float> wt, bias;
+};
+
+// Reads conv weight [cout][cin][k][k] (+ optional BN gamma, beta, mean, var) and uploads the folded tensors: transposed for the
+// SIMT kernel and, where eligible, split for both tensor-core arithmetics.  Fold: y = (conv - mean) / sqrt(var + 1e-5) * gamma + beta
+// (net/resnet50.py:11-14).  `host`, if given, receives the folded weights for the callers that repack them.
+static int read_conv(DeviceAllocs& mem, Reader& rd, Conv& c, int cin, int cout, int k, int stride, int pad, bool bn,
+                     HostWeights* host = nullptr) {
     c.cin = cin; c.cout = cout; c.k = k; c.stride = stride; c.pad = pad;
     const size_t nw = (size_t)cout * cin * k * k;
     const float* w = rd.take(nw);
@@ -134,194 +215,94 @@ static int read_conv(irn_net* net, Reader& rd, Conv& c, int cin, int cout, int k
             for (int r = 0; r < k; ++r)
                 for (int s = 0; s < k; ++s)
                     wt[((size_t)(r * k + s) * cin + ci) * cout + o] = (float)((double)w[(((size_t)o * cin + ci) * k + r) * k + s] * scale[o]);
-    int rc = upload(net, wt, &c.wt);
+    int rc = upload(mem, wt, &c.wt);
     if (rc) return rc;
-    if (bn && (rc = upload(net, bias, &c.bias))) return rc;
-    c.host_wt = wt;
-    c.host_bias = bias;
-    if ((rc = make_bf16_weights(net, c, wt))) return rc;
-    // tensor-core eligibility: 32-channel k slices, 64/128-wide N tiles, 1x1 or 3x3, stride 1 or 2
-    c.bn = (cout % 128 == 0) ? 128 : (cout % 64 == 0 ? 64 : 0);
-    if (cin % kTcBK != 0 || !(k == 1 || k == 3) || !(stride == 1 || stride == 2)) c.bn = 0;
-    if (c.bn) {
-        const size_t K = (size_t)k * k * cin;
-        std::vector<float> hi(nw), lo(nw);
-        for (int o = 0; o < cout; ++o)
-            for (size_t kk = 0; kk < K; ++kk) {
-                const float v = wt[kk * cout + o];
-                uint32_t u;
-                std::memcpy(&u, &v, 4);
-                // round-to-nearest (ties away) to 10 explicit mantissa bits, like cvt.rna.tf32.f32
-                uint32_t h = (u + 0x1000u) & 0xFFFFE000u;
-                float hf;
-                std::memcpy(&hf, &h, 4);
-                if (!std::isfinite(hf)) hf = v;
-                hi[(size_t)o * K + kk] = hf;
-                lo[(size_t)o * K + kk] = v - hf;
-            }
-        if ((rc = upload(net, hi, &c.w_hi))) return rc;
-        if ((rc = upload(net, lo, &c.w_lo))) return rc;
-        const uint64_t dims[2] = {(uint64_t)K, (uint64_t)cout};
-        const uint64_t strides[1] = {(uint64_t)K * sizeof(float)};
-        const uint32_t box[2] = {(uint32_t)kTcBK, (uint32_t)c.bn};
-        if ((rc = make_tensor_map(&c.map_bhi, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c.w_hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-        if ((rc = make_tensor_map(&c.map_blo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c.w_lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
+    if (bn && (rc = upload(mem, bias, &c.bias))) return rc;
+    const size_t K = (size_t)k * k * cin;
+    if (split_eligible(cin, cout, k, stride, kBfBK) && (rc = pack_split(mem, true, wt.data(), K, cout, c.f16))) return rc;
+    if (split_eligible(cin, cout, k, stride, kTcBK) && (rc = pack_split(mem, false, wt.data(), K, cout, c.tf32))) return rc;
+    if (host) {
+        host->wt = std::move(wt);
+        host->bias = std::move(bias);
     }
     return kOk;
 }
 
-// fp16 hi / lo planes of the folded weights, [cout][K] K-major, + tensor maps for 64- / 128-row tiles.  Every output
-// channel is first scaled by a power of two so that max |w| lies in [1,2): the lo parts stay clear of fp16's subnormal range
-// whatever FixedBatchNorm's gamma / sqrt(var) did to the channel, and the epilogue undoes the scale exactly.
-static int make_bf16_weights(irn_net* net, Conv& c, const std::vector<float>& wt /* [K][cout] */) {
-    const size_t K = (size_t)c.k * c.k * c.cin;
-    c.bf_ok = c.cin % kBfBK == 0 && c.cout % 64 == 0 && (c.k == 1 || c.k == 3) && (c.stride == 1 || c.stride == 2);
-    if (!c.bf_ok) return kOk;
-    std::vector<uint16_t> hi((size_t)c.cout * K), lo((size_t)c.cout * K);
-    std::vector<float> inv(c.cout, 1.0f);
-    for (int o = 0; o < c.cout; ++o) {
-        float mx = 0.f;
-        for (size_t kk = 0; kk < K; ++kk) mx = std::max(mx, std::fabs(wt[kk * c.cout + o]));
-        int e = 1;
-        if (mx > 0.f && std::isfinite(mx)) std::frexp(mx, &e);          // mx = m * 2^e, m in [0.5, 1)
-        const int sh = 1 - e;                                           // w * 2^sh has its maximum in [1, 2)
-        inv[o] = std::ldexp(1.0f, -sh);
-        for (size_t kk = 0; kk < K; ++kk) {
-            const float v = std::ldexp(wt[kk * c.cout + o], sh);
-            const __half h = __float2half_rn(v);
-            const __half l = __float2half_rn(v - __half2float(h));
-            hi[(size_t)o * K + kk] = __half_as_ushort(h);
-            lo[(size_t)o * K + kk] = __half_as_ushort(l);
-        }
-    }
-    int rc = upload(net, inv, &c.oscale);
-    if (rc) return rc;
-    for (int part = 0; part < 2; ++part) {
-        void* d = nullptr;
-        IRN_CUDA(cudaMalloc(&d, hi.size() * sizeof(uint16_t)));
-        net->allocs.push_back(d);
-        IRN_CUDA(cudaMemcpy(d, part == 0 ? hi.data() : lo.data(), hi.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-        (part == 0 ? c.wb_hi : c.wb_lo) = (uint16_t*)d;
-    }
-    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)c.cout};
-    const uint64_t strides[1] = {(uint64_t)K * sizeof(uint16_t)};
-    for (int i = 0; i < 2; ++i) {
-        const uint32_t rows = 64u << i;
-        if (c.cout % rows != 0) continue;
-        const uint32_t box[2] = {(uint32_t)kBfBK, rows};
-        if ((rc = make_tensor_map(&c.map_bf_hi[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, c.wb_hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-        if ((rc = make_tensor_map(&c.map_bf_lo[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, c.wb_lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-    }
-    return kOk;
-}
-
-static int read_vec(irn_net* net, Reader& rd, size_t n, float** out) {
+static int read_vec(DeviceAllocs& mem, Reader& rd, size_t n, float** out) {
     const float* p = rd.take(n);
     if (!rd.ok) return fail(kBadArg, "parameter blob too short (vector of %zu)", n);
-    return upload(net, std::vector<float>(p, p + n), out);
+    return upload(mem, std::vector<float>(p, p + n), out);
 }
 
-// Repacks the folded 7x7/s2 stem (read_conv'd into `c`) for the tensor-core kernels over the zero-haloed NHWC4 input: the 3xTF32
-// planes of `c` and the f16x3 conv `f`
-static int build_stem(irn_net* net, Conv& c, Conv& f) {
-    int rc;
-    {   // tensor-core stem: K = 7 rows x (8 taps x 4 channels) = 224, tap 7 and channel 3 carry zero weights
-        std::vector<float> host((size_t)49 * 3 * 64);
-        IRN_CUDA(cudaMemcpy(host.data(), c.wt, host.size() * sizeof(float), cudaMemcpyDeviceToHost));
-        const size_t K = 224;
-        std::vector<float> hi(64 * K, 0.f), lo(64 * K, 0.f);
-        for (int o = 0; o < 64; ++o)
-            for (int r = 0; r < 7; ++r)
-                for (int t = 0; t < 7; ++t)
-                    for (int ci = 0; ci < 3; ++ci) {
-                        const float v = host[((size_t)(r * 7 + t) * 3 + ci) * 64 + o];
-                        uint32_t u;
-                        std::memcpy(&u, &v, 4);
-                        uint32_t h = (u + 0x1000u) & 0xFFFFE000u;
-                        float hf;
-                        std::memcpy(&hf, &h, 4);
-                        if (!std::isfinite(hf)) hf = v;
-                        hi[(size_t)o * K + r * 32 + t * 4 + ci] = hf;
-                        lo[(size_t)o * K + r * 32 + t * 4 + ci] = v - hf;
-                    }
-        if ((rc = upload(net, hi, &c.w_hi))) return rc;
-        if ((rc = upload(net, lo, &c.w_lo))) return rc;
-        const uint64_t dims[2] = {K, 64};
-        const uint64_t strides[1] = {K * sizeof(float)};
-        const uint32_t box[2] = {(uint32_t)kTcBK, 64};
-        if ((rc = make_tensor_map(&c.map_bhi, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c.w_hi, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-        if ((rc = make_tensor_map(&c.map_blo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c.w_lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-        c.stem_tc = true;
-        // f16x3 stem: the same rows, K = 8 filter rows x 32 (row 7 zero) = 256 = four 64-wide k-blocks
-        f.cin = 256; f.cout = 64; f.k = 1; f.stride = 1; f.pad = 0;
-        std::vector<float> wt((size_t)256 * 64, 0.f);
-        for (int o = 0; o < 64; ++o)
-            for (int r = 0; r < 7; ++r)
-                for (int t = 0; t < 7; ++t)
-                    for (int ci = 0; ci < 3; ++ci)
-                        wt[(size_t)(r * 32 + t * 4 + ci) * 64 + o] = host[((size_t)(r * 7 + t) * 3 + ci) * 64 + o];
-        f.bias = c.bias;
-        if ((rc = make_bf16_weights(net, f, wt))) return rc;
-    }
-    return kOk;
+// Splits the stem's folded 7x7x3 weights (wt [49*3][64] from read_conv) for the tensor-core kernel over the zero-haloed NHWC4 input:
+// filter row r, tap t, channel ci at k = r*32 + t*4 + ci, tap 7 and channel 3 zero.  3xTF32: K = 7 rows x 32 = 224, one filter row
+// per k-block; f16x3: K = 8 rows x 32 = 256 (row 7 zero), four 64-wide k-blocks.
+static int build_stem(DeviceAllocs& mem, Conv& c, const std::vector<float>& wt) {
+    std::vector<float> rows((size_t)256 * 64, 0.f);
+    for (int o = 0; o < 64; ++o)
+        for (int r = 0; r < 7; ++r)
+            for (int t = 0; t < 7; ++t)
+                for (int ci = 0; ci < 3; ++ci)
+                    rows[(size_t)(r * 32 + t * 4 + ci) * 64 + o] = wt[((size_t)(r * 7 + t) * 3 + ci) * 64 + o];
+    int rc = pack_split(mem, false, rows.data(), 224, 64, c.tf32);
+    if (rc) return rc;
+    return pack_split(mem, true, rows.data(), 256, 64, c.f16);
 }
 
-// f16x3 mode: conv3 and the projection shortcut of a first block (both read_conv'd with BN, host copies still present) as one
-// K-concatenated 1x1 conv; blk.has_c3ds says whether it was eligible
-static int build_c3ds(irn_net* net, Block& blk, int cin, int planes) {
+// The fused conv3 + projection shortcut reads both inputs in whole f16x3 k-blocks
+static bool c3ds_eligible(int planes, int cin, int stride) {
+    return split_eligible(planes, 4 * planes, 1, 1, kBfBK) && split_eligible(cin, 4 * planes, 1, stride, kBfBK);
+}
+
+// f16x3 mode: conv3 and the projection shortcut of a first block (blk.c3 and blk.ds read with BN, h3 and hds their folded host
+// weights) as one K-concatenated 1x1 conv; blk.has_c3ds says whether it was eligible
+static int build_c3ds(DeviceAllocs& mem, Block& blk, const HostWeights& h3, const HostWeights& hds) {
+    const int planes = blk.c3.cin, cin = blk.ds.cin, cout = blk.c3.cout;
     blk.has_c3ds = false;
-    if (planes % kBfBK != 0 || cin % kBfBK != 0) return kOk;
+    if (!c3ds_eligible(planes, cin, blk.ds.stride)) return kOk;
     Conv& f = blk.c3ds;
-    const int cout = planes * 4, K3 = planes, Kd = cin;
-    f.cin = K3 + Kd; f.cout = cout; f.k = 1; f.stride = 1; f.pad = 0;
-    std::vector<float> wt((size_t)(K3 + Kd) * cout), bias(cout);
-    std::copy(blk.c3.host_wt.begin(), blk.c3.host_wt.end(), wt.begin());
-    std::copy(blk.ds.host_wt.begin(), blk.ds.host_wt.end(), wt.begin() + (size_t)K3 * cout);
-    for (int o = 0; o < cout; ++o) bias[o] = blk.c3.host_bias[o] + blk.ds.host_bias[o];
+    f.cin = planes + cin; f.cout = cout; f.k = 1; f.stride = 1; f.pad = 0;
+    std::vector<float> wt(h3.wt), bias(cout);
+    wt.insert(wt.end(), hds.wt.begin(), hds.wt.end());
+    for (int o = 0; o < cout; ++o) bias[o] = h3.bias[o] + hds.bias[o];
     int rc;
-    if ((rc = upload(net, bias, &f.bias))) return rc;
-    if ((rc = make_bf16_weights(net, f, wt))) return rc;
-    blk.has_c3ds = f.bf_ok;
+    if ((rc = upload(mem, bias, &f.bias))) return rc;
+    if ((rc = pack_split(mem, true, wt.data(), f.cin, cout, f.f16))) return rc;
+    blk.has_c3ds = true;
     return kOk;
 }
 
 static int read_trunk(irn_net* net, Reader& rd) {
-    int rc = read_conv(net, rd, net->stem, 3, 64, 7, 2, 3, true);
+    HostWeights stem;
+    int rc = read_conv(net->mem, rd, net->stem, 3, 64, 7, 2, 3, true, &stem);
     if (rc) return rc;
-    if ((rc = build_stem(net, net->stem, net->stem_f16))) return rc;
+    if ((rc = build_stem(net->mem, net->stem, stem.wt))) return rc;
     int cin = 64;
     for (int l = 0; l < 4; ++l) {
         net->blocks[l].resize(kBlocks[l]);
         for (int b = 0; b < kBlocks[l]; ++b) {
             Block& blk = net->blocks[l][b];
             const int planes = kPlanes[l], stride = b == 0 ? kStrides[l] : 1;
-            if ((rc = read_conv(net, rd, blk.c1, cin, planes, 1, 1, 0, true))) return rc;
-            if ((rc = read_conv(net, rd, blk.c2, planes, planes, 3, stride, 1, true))) return rc;   // stride on conv2 (net/resnet50.py:24)
-            if ((rc = read_conv(net, rd, blk.c3, planes, planes * 4, 1, 1, 0, true))) return rc;
+            HostWeights h3, hds;
+            if ((rc = read_conv(net->mem, rd, blk.c1, cin, planes, 1, 1, 0, true))) return rc;
+            if ((rc = read_conv(net->mem, rd, blk.c2, planes, planes, 3, stride, 1, true))) return rc;   // stride on conv2 (net/resnet50.py:24)
+            if ((rc = read_conv(net->mem, rd, blk.c3, planes, planes * 4, 1, 1, 0, true, &h3))) return rc;
             blk.has_ds = b == 0;
-            if (blk.has_ds && (rc = read_conv(net, rd, blk.ds, cin, planes * 4, 1, stride, 0, true))) return rc;
-            if (blk.has_ds && (rc = build_c3ds(net, blk, cin, planes))) return rc;
+            if (blk.has_ds && (rc = read_conv(net->mem, rd, blk.ds, cin, planes * 4, 1, stride, 0, true, &hds))) return rc;
+            if (blk.has_ds && (rc = build_c3ds(net->mem, blk, h3, hds))) return rc;
             cin = planes * 4;
         }
     }
-    // the host copies were only needed to build the fused convs
-    net->stem.host_wt.clear(); net->stem.host_wt.shrink_to_fit();
-    for (int l = 0; l < 4; ++l)
-        for (Block& blk : net->blocks[l])
-            for (Conv* c : {&blk.c1, &blk.c2, &blk.c3, &blk.ds}) {
-                std::vector<float>().swap(c->host_wt);
-                std::vector<float>().swap(c->host_bias);
-            }
     return kOk;
 }
 
-static int read_head(irn_net* net, Reader& rd, Head& h, int cin, int cout, int groups, int up) {
-    int rc = read_conv(net, rd, h.conv, cin, cout, 1, 1, 0, false);
+static int read_head(DeviceAllocs& mem, Reader& rd, Head& h, int cin, int cout, int groups, int up) {
+    int rc = read_conv(mem, rd, h.conv, cin, cout, 1, 1, 0, false);
     if (rc) return rc;
     h.groups = groups;
     h.up = up;
-    if ((rc = read_vec(net, rd, cout, &h.gamma))) return rc;
-    return read_vec(net, rd, cout, &h.beta);
+    if ((rc = read_vec(mem, rd, cout, &h.gamma))) return rc;
+    return read_vec(mem, rd, cout, &h.beta);
 }
 
 // ------------------------------------------------------------------ launch helpers
@@ -353,7 +334,6 @@ static int launch_wg(const TcMaps& maps, const TcArgs& a, cudaStream_t st) {
 static TcArgs conv_args(const Conv& c, int B, int Ho, int Wo, const float* residual, float* out, bool relu) {
     TcArgs a;
     a.bias = c.bias; a.residual = residual; a.out = out;
-    a.oscale = c.oscale;
     a.B = B; a.Ho = Ho; a.Wo = Wo; a.Cout = c.cout; a.Cin = c.cin; a.ksize = c.k; a.stride = c.stride; a.pad = c.pad;
     a.relu = relu ? 1 : 0;
     a.tiles_x = (Wo + kTcTW - 1) / kTcTW;
@@ -382,75 +362,22 @@ static int stem_map(CUtensorMap* m, const float* x4, int B, int Hin, int Win) {
     return make_tensor_map(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, x4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, estr);
 }
 
-// 3xTF32 convolution (eligible when c.bn != 0)
-static int run_conv_tf32(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out, bool relu,
-                         cudaStream_t st) {
+// The tensor-core convolution in one arithmetic: weights `w` (f16x3 or 3xTF32 split, as `f16` says), activations through `act` and,
+// for a K-concatenated conv (a.kb_split), `act2`; N tile 128 when it divides Cout, else 64
+static int launch_tc(bool f16, const SplitWeights& w, const CUtensorMap& act, const CUtensorMap* act2, TcArgs a, cudaStream_t st) {
+    const bool wide = a.Cout % 128 == 0;
     TcMaps maps;
-    maps.b_hi = c.map_bhi;
-    maps.b_lo = c.map_blo;
-    int rc = act_map(&maps.a, in, B, H, W, c.cin, c.stride);
-    if (rc) return rc;
-    maps.a2 = maps.a;
-    TcArgs a = conv_args(c, B, Ho, Wo, residual, out, relu);
-    a.oscale = nullptr;
-    return c.bn == 128 ? launch_wg<false, 128>(maps, a, st) : launch_wg<false, 64>(maps, a, st);
+    maps.a = act;
+    maps.a2 = act2 ? *act2 : act;
+    maps.b_hi = w.map_hi[wide ? 1 : 0];
+    maps.b_lo = w.map_lo[wide ? 1 : 0];
+    a.oscale = f16 ? w.oscale : nullptr;
+    if (f16) return wide ? launch_wg<true, 128>(maps, a, st) : launch_wg<true, 64>(maps, a, st);
+    return wide ? launch_wg<false, 128>(maps, a, st) : launch_wg<false, 64>(maps, a, st);
 }
 
-// 3xTF32 stem: K = 7 filter rows x (8 taps x 4 channels), out NHWC [B,Ho,Wo,64] with bias + ReLU
-static int launch_tf32_stem(const Conv& c, const float* x4, int B, int Hin, int Win, float* out, cudaStream_t st) {
-    TcMaps maps;
-    maps.b_hi = c.map_bhi;
-    maps.b_lo = c.map_blo;
-    int rc = stem_map(&maps.a, x4, B, Hin, Win);
-    if (rc) return rc;
-    maps.a2 = maps.a;
-    TcArgs a = conv_args(c, B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), nullptr, out, true);
-    a.oscale = nullptr;
-    a.Cin = 32; a.ksize = 7; a.stride = 2; a.pad = 3; a.stem = 1;
-    return launch_wg<false, 64>(maps, a, st);
-}
-
-// Second input of a K-concatenated 1x1 conv (Block::c3ds): NHWC [B, H2, W2, cin2] sampled with pixel stride `stride`
-struct F16Second {
-    const float* in = nullptr;
-    int H = 0, W = 0, cin = 0, stride = 1;
-};
-
-// f16x3 convolution (eligible when c.bf_ok)
-static int run_conv_f16(const Conv& c, const float* in, int B, int H, int W, int Ho, int Wo, const float* residual, float* out, bool relu,
-                        cudaStream_t st, const F16Second* second = nullptr) {
-    const bool wide = c.cout % 128 == 0;
-    TcMaps maps;
-    maps.b_hi = c.map_bf_hi[wide ? 1 : 0];
-    maps.b_lo = c.map_bf_lo[wide ? 1 : 0];
-    const int cin1 = second ? c.cin - second->cin : c.cin;        // channels of the first input
-    int rc = act_map(&maps.a, in, B, H, W, cin1, c.stride);
-    if (rc) return rc;
-    maps.a2 = maps.a;
-    TcArgs a = conv_args(c, B, Ho, Wo, residual, out, relu);
-    if (second) {
-        if (c.k != 1) return fail(kUnsupported, "run_conv_f16: a second input needs a 1x1 conv");
-        if ((rc = act_map(&maps.a2, second->in, B, second->H, second->W, second->cin, second->stride))) return rc;
-        a.kb_split = cin1 / kBfBK;
-        a.stride2 = second->stride;
-    }
-    return wide ? launch_wg<true, 128>(maps, a, st) : launch_wg<true, 64>(maps, a, st);
-}
-
-// f16x3 stem: the same rows as the 3xTF32 stem, K = 8 filter rows x 32 (row 7 zero) = four 64-wide k-blocks
-static int launch_f16_stem(const Conv& c, const float* x4, int B, int Hin, int Win, float* out, cudaStream_t st) {
-    TcMaps maps;
-    maps.b_hi = c.map_bf_hi[0];
-    maps.b_lo = c.map_bf_lo[0];
-    int rc = stem_map(&maps.a, x4, B, Hin, Win);
-    if (rc) return rc;
-    maps.a2 = maps.a;
-    TcArgs a = conv_args(c, B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), nullptr, out, true);
-    a.Cin = 256; a.ksize = 1; a.stride = 2; a.pad = 0; a.stem = 1;
-    return launch_wg<true, 64>(maps, a, st);
-}
-
-static int run_conv(const irn_net* net, const Conv& c, const float* in, int B, int H, int W, const float* residual, float* out, bool relu,
+// One conv in `mode` (as irn_net_set_conv_mode): the f16x3 or 3xTF32 tensor-core kernel where the conv is eligible, SIMT otherwise
+static int run_conv(int mode, const Conv& c, const float* in, int B, int H, int W, const float* residual, float* out, bool relu,
                     cudaStream_t st, int* Ho_, int* Wo_) {
     ConvGeom g;
     g.B = B; g.H = H; g.W = W; g.Cin = c.cin;
@@ -459,8 +386,13 @@ static int run_conv(const irn_net* net, const Conv& c, const float* in, int B, i
     g.Cout = c.cout; g.k = c.k; g.stride = c.stride; g.pad = c.pad;
     if (Ho_) *Ho_ = g.Ho;
     if (Wo_) *Wo_ = g.Wo;
-    if (net->conv_mode == 2 && c.bf_ok) return run_conv_f16(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
-    if (net->conv_mode >= 1 && c.bn) return run_conv_tf32(c, in, B, H, W, g.Ho, g.Wo, residual, out, relu, st);
+    const SplitWeights* sw = mode == 2 && c.f16.ok ? &c.f16 : mode >= 1 && c.tf32.ok ? &c.tf32 : nullptr;
+    if (sw) {
+        CUtensorMap act;
+        int rc = act_map(&act, in, B, H, W, c.cin, c.stride);
+        if (rc) return rc;
+        return launch_tc(sw == &c.f16, *sw, act, nullptr, conv_args(c, B, g.Ho, g.Wo, residual, out, relu), st);
+    }
     const int M = B * g.Ho * g.Wo;
     dim3 grid((M + kBM - 1) / kBM, (c.cout + kBN - 1) / kBN);
     if (c.cin % 16 == 0)
@@ -513,36 +445,50 @@ static TrunkShapes trunk_shapes(int B, int H, int W) {
 // conv3 + projection shortcut in one reduction (Block::c3ds): out = relu([W3 | Wds] . [t2 ; x sampled at the block's stride] + b3 + bds),
 // x NHWC on the block's input grid h x w, t2 and out on its output grid ho x wo
 static int run_c3ds(const Block& blk, const float* t2, const float* x, int B, int h, int w, int ho, int wo, float* out, cudaStream_t st) {
-    F16Second sec;
-    sec.in = x; sec.H = h; sec.W = w; sec.cin = blk.ds.cin; sec.stride = blk.ds.stride;
-    return run_conv_f16(blk.c3ds, t2, B, ho, wo, ho, wo, nullptr, out, true, st, &sec);
+    const Conv& f = blk.c3ds;
+    const int cin1 = f.cin - blk.ds.cin;   // channels of t2
+    CUtensorMap act, act2;
+    int rc = act_map(&act, t2, B, ho, wo, cin1, f.stride);
+    if (rc) return rc;
+    if ((rc = act_map(&act2, x, B, h, w, blk.ds.cin, blk.ds.stride))) return rc;
+    TcArgs a = conv_args(f, B, ho, wo, nullptr, out, true);
+    a.kb_split = cin1 / kBfBK;
+    a.stride2 = blk.ds.stride;
+    return launch_tc(true, f.f16, act, &act2, a, st);
 }
 
-static bool stem_on_tensor_cores(const irn_net* net) { return net->conv_mode >= 1 && net->stem.stem_tc; }
+// floats of the zero-haloed NHWC4 stem input of the tensor-core stems, the larger of run_stem's two input layouts
+static size_t stem_halo_floats(int B, int Hin, int Win) { return (size_t)B * (Hin + 6) * (Win + 8) * 4; }
 
 // floats of run_stem's input buffer x_in: the zero-haloed NHWC4 layout for the tensor-core stems, plain NHWC otherwise
-static size_t stem_input_floats(const irn_net* net, int B, int Hin, int Win) {
-    return stem_on_tensor_cores(net) ? (size_t)B * (Hin + 6) * (Win + 8) * 4 : (size_t)B * Hin * Win * 3;
+static size_t stem_input_floats(int mode, int B, int Hin, int Win) {
+    return mode >= 1 ? stem_halo_floats(B, Hin, Win) : (size_t)B * Hin * Win * 3;
 }
 
-// The stem of the trunk: x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win is laid out in x_in (stem_input_floats), then
-// conv 7x7/s2 + bias + ReLU -> out NHWC [B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), 64]
-static int run_stem(const irn_net* net, const float* x_nchw, int B, int H, int W, int Hin, int Win, float* x_in, float* out,
+// The stem (`c`, built by build_stem) in `mode`: x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win is laid out in x_in
+// (stem_input_floats), then conv 7x7/s2 + bias + ReLU -> out NHWC [B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), 64]
+static int run_stem(int mode, const Conv& c, const float* x_nchw, int B, int H, int W, int Hin, int Win, float* x_in, float* out,
                     cudaStream_t st) {
-    int rc;
-    if (stem_on_tensor_cores(net)) {
+    if (mode >= 1) {
         const size_t total = (size_t)B * (Hin + 6) * (Win + 8);
         nchw_to_nhwc4_halo_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, (float4*)x_in, B, H, W, Hin + 6, Win + 8);
         IRN_LAUNCH_CHECK("nchw_to_nhwc4_halo_kernel");
-        static const int stem_f16 = getenv("IRN_F16_STEM") ? atoi(getenv("IRN_F16_STEM")) : 1;
-        if (net->conv_mode == 2 && net->stem_f16.bf_ok && stem_f16) return launch_f16_stem(net->stem_f16, x_in, B, Hin, Win, out, st);
-        return launch_tf32_stem(net->stem, x_in, B, Hin, Win, out, st);
+        CUtensorMap act;
+        int rc = stem_map(&act, x_in, B, Hin, Win);
+        if (rc) return rc;
+        TcArgs a = conv_args(c, B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), nullptr, out, true);
+        a.stem = 1;
+        if (mode == 2) {   // f16x3: K = 8 filter rows x 32 = four 64-wide k-blocks
+            a.Cin = 256; a.ksize = 1; a.pad = 0;
+            return launch_tc(true, c.f16, act, nullptr, a, st);
+        }
+        a.Cin = 32;        // 3xTF32: one filter row of 8 taps x 4 channels per k-block
+        return launch_tc(false, c.tf32, act, nullptr, a, st);
     }
     const size_t total = (size_t)B * Hin * Win * 3;
     nchw_to_nhwc_pad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, x_in, B, 3, H, W, Hin, Win);
     IRN_LAUNCH_CHECK("nchw_to_nhwc_pad_kernel");
-    if ((rc = run_conv(net, net->stem, x_in, B, Hin, Win, nullptr, out, true, st, nullptr, nullptr))) return rc;
-    return kOk;
+    return run_conv(0, c, x_in, B, Hin, Win, nullptr, out, true, st, nullptr, nullptr);
 }
 
 // Runs input layout transform + stem + maxpool + layer1..4 on x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win.
@@ -551,7 +497,7 @@ static int run_stem(const irn_net* net, const float* x_nchw, int B, int H, int W
 static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int W, int Hin, int Win, Arena& ar, bool keep,
                      const float* feats[5], TrunkShapes& sh, cudaStream_t st) {
     sh = trunk_shapes(B, Hin, Win);
-    float* x_in = ar.take(stem_input_floats(net, B, Hin, Win));
+    float* x_in = ar.take(stem_input_floats(net->conv_mode, B, Hin, Win));
     float* stem_out = ar.take((size_t)B * sh.H1 * sh.W1 * 64);
     float* pool_out = ar.take((size_t)B * sh.H2 * sh.W2 * 64);
     float* t1 = ar.take(sh.max_act);
@@ -560,7 +506,7 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
     float* ping[2] = {ar.take(sh.max_act), ar.take(sh.max_act)};
     if (!ar.ok) return fail(kWorkspace, "network workspace too small");
     int rc;
-    if ((rc = run_stem(net, x_nchw, B, H, W, Hin, Win, x_in, stem_out, st))) return rc;
+    if ((rc = run_stem(net->conv_mode, net->stem, x_nchw, B, H, W, Hin, Win, x_in, stem_out, st))) return rc;
     {
         const size_t total = (size_t)B * sh.H2 * sh.W2 * 16;
         maxpool3s2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(stem_out, pool_out, B, sh.H1, sh.W1, 64, sh.H2, sh.W2);
@@ -574,13 +520,12 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
         for (int b = 0; b < nb; ++b) {
             const Block& blk = net->blocks[l][b];
             int ho, wo;
-            if ((rc = run_conv(net, blk.c1, x, B, h, w, nullptr, t1, true, st, nullptr, nullptr))) return rc;
-            if ((rc = run_conv(net, blk.c2, t1, B, h, w, nullptr, t2, true, st, &ho, &wo))) return rc;
-            static const int fuse_ds = getenv("IRN_F16_FUSE_DS") ? atoi(getenv("IRN_F16_FUSE_DS")) : 1;
-            const bool fused = net->conv_mode == 2 && blk.has_c3ds && fuse_ds;
+            if ((rc = run_conv(net->conv_mode, blk.c1, x, B, h, w, nullptr, t1, true, st, nullptr, nullptr))) return rc;
+            if ((rc = run_conv(net->conv_mode, blk.c2, t1, B, h, w, nullptr, t2, true, st, &ho, &wo))) return rc;
+            const bool fused = net->conv_mode == 2 && blk.has_c3ds;
             const float* res = x;
             if (blk.has_ds && !fused) {
-                if ((rc = run_conv(net, blk.ds, x, B, h, w, nullptr, dsb, false, st, nullptr, nullptr))) return rc;
+                if ((rc = run_conv(net->conv_mode, blk.ds, x, B, h, w, nullptr, dsb, false, st, nullptr, nullptr))) return rc;
                 res = dsb;
             }
             float* out;
@@ -593,7 +538,7 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
             }
             if (fused) {
                 if ((rc = run_c3ds(blk, t2, x, B, h, w, ho, wo, out, st))) return rc;
-            } else if ((rc = run_conv(net, blk.c3, t2, B, ho, wo, res, out, true, st, nullptr, nullptr))) return rc;   // out += residual; relu (net/resnet50.py:51-52)
+            } else if ((rc = run_conv(net->conv_mode, blk.c3, t2, B, ho, wo, res, out, true, st, nullptr, nullptr))) return rc;   // out += residual; relu (net/resnet50.py:51-52)
             x = out;
             h = ho;
             w = wo;
@@ -605,7 +550,7 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
 
 static size_t trunk_workspace_floats(int B, int H, int W, bool keep) {
     TrunkShapes s = trunk_shapes(B, H, W);
-    size_t n = (size_t)B * (H + 6) * (W + 8) * 4 + (size_t)B * s.H1 * s.W1 * 64 + (size_t)B * s.H2 * s.W2 * 64 + 5 * s.max_act;
+    size_t n = stem_halo_floats(B, H, W) + (size_t)B * s.H1 * s.W1 * 64 + (size_t)B * s.H2 * s.W2 * 64 + 5 * s.max_act;
     if (keep)
         for (int l = 0; l < 4; ++l) n += (size_t)B * s.Hl[l] * s.Wl[l] * kPlanes[l] * 4;
     return n + 64 * 32;   // alignment slack (256 B per buffer)
@@ -615,10 +560,14 @@ static size_t trunk_workspace_floats(int B, int H, int W, bool keep) {
 
 using namespace irn;
 
-// ---- single convolution as a plan of its own (unit tests / integration of other networks)
+// ---- single convolution as a plan of its own (unit tests / integration of other networks).  A handle is of one kind, set by the
+// call that created it, and each forward call refuses the other kinds.
 struct irn_conv {
-    irn_net holder;   // owns the device allocations
-    irn::Conv conv;
+    enum Kind { kConv, kStem, kShortcut } kind;
+    irn::DeviceAllocs mem;
+    irn::Conv conv;     // kConv; kStem: the stem with its repacked splits (build_stem)
+    irn::Block block;   // kShortcut: c3, ds and the fused c3ds (build_c3ds)
+    explicit irn_conv(Kind k) : kind(k) {}
 };
 
 extern "C" int irn_conv_create(const float* weight_oihw, const float* bn4 /* gamma,beta,mean,var or NULL */, int cin, int cout, int k,
@@ -627,11 +576,10 @@ extern "C" int irn_conv_create(const float* weight_oihw, const float* bn4 /* gam
     const size_t nw = (size_t)cout * cin * k * k;
     std::vector<float> blob(weight_oihw, weight_oihw + nw);
     if (bn4) blob.insert(blob.end(), bn4, bn4 + 4 * (size_t)cout);
-    irn_conv* c = new irn_conv();
+    irn_conv* c = new irn_conv(irn_conv::kConv);
     Reader rd{blob.data(), blob.size()};
-    int rc = read_conv(&c->holder, rd, c->conv, cin, cout, k, stride, pad, bn4 != nullptr);
+    int rc = read_conv(c->mem, rd, c->conv, cin, cout, k, stride, pad, bn4 != nullptr);
     if (rc) {
-        for (void* p : c->holder.allocs) cudaFree(p);
         delete c;
         return rc;
     }
@@ -639,23 +587,20 @@ extern "C" int irn_conv_create(const float* weight_oihw, const float* bn4 /* gam
     return kOk;
 }
 
-extern "C" void irn_conv_destroy(irn_conv* c) {
-    if (!c) return;
-    for (void* p : c->holder.allocs) cudaFree(p);
-    delete c;
-}
+extern "C" void irn_conv_destroy(irn_conv* c) { delete c; }
 
 // The network's stem as a plan of its own, built and run by the same code as the trunk's (build_stem, run_stem)
 extern "C" int irn_stem_create(const float* weight_oihw, const float* bn4, irn_conv** out) {
     if (!weight_oihw || !out) return fail(kBadArg, "irn_stem_create: bad argument");
     std::vector<float> blob(weight_oihw, weight_oihw + (size_t)64 * 3 * 7 * 7);
     if (bn4) blob.insert(blob.end(), bn4, bn4 + 4 * 64);
-    irn_conv* c = new irn_conv();
+    irn_conv* c = new irn_conv(irn_conv::kStem);
     Reader rd{blob.data(), blob.size()};
-    int rc = read_conv(&c->holder, rd, c->holder.stem, 3, 64, 7, 2, 3, bn4 != nullptr);
-    if (!rc) rc = build_stem(&c->holder, c->holder.stem, c->holder.stem_f16);
+    HostWeights host;
+    int rc = read_conv(c->mem, rd, c->conv, 3, 64, 7, 2, 3, bn4 != nullptr, &host);
+    if (!rc) rc = build_stem(c->mem, c->conv, host.wt);
     if (rc) {
-        irn_conv_destroy(c);
+        delete c;
         return rc;
     }
     *out = c;
@@ -664,20 +609,20 @@ extern "C" int irn_stem_create(const float* weight_oihw, const float* bn4, irn_c
 
 extern "C" size_t irn_stem_workspace_bytes(int B, int Hin, int Win) {
     if (B <= 0 || Hin <= 0 || Win <= 0) return 0;
-    return (size_t)B * (Hin + 6) * (Win + 8) * 4 * sizeof(float);   // the larger of the two stem_input_floats layouts
+    return stem_halo_floats(B, Hin, Win) * sizeof(float);   // the larger of the two stem_input_floats layouts
 }
 
 extern "C" int irn_stem_forward(irn_conv* c, const float* x_nchw, int B, int H, int W, int Hin, int Win, float* out_nhwc, int mode,
                                 void* workspace, size_t workspace_bytes, irn_stream_t stream) {
     launch_counter() = 0;
-    if (!c || !c->holder.stem.stem_tc || !x_nchw || !out_nhwc || !workspace) return fail(kBadArg, "irn_stem_forward: bad argument");
+    if (!c || c->kind != irn_conv::kStem) return fail(kBadArg, "irn_stem_forward: not a handle from irn_stem_create");
+    if (!x_nchw || !out_nhwc || !workspace) return fail(kBadArg, "irn_stem_forward: bad argument");
     if (B <= 0 || H <= 0 || W <= 0 || H > Hin || W > Win)
         return fail(kBadArg, "irn_stem_forward: need B > 0 and 0 < H <= Hin, 0 < W <= Win; got B=%d H=%d W=%d Hin=%d Win=%d", B, H, W, Hin, Win);
     if (mode < 0 || mode > 2) return fail(kBadArg, "irn_stem_forward: mode must be 0, 1 or 2");
     if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "irn_stem_forward: workspace must be 256-byte aligned");
     if (workspace_bytes < irn_stem_workspace_bytes(B, Hin, Win)) return fail(kWorkspace, "irn_stem_forward: workspace too small");
-    c->holder.conv_mode = mode;
-    return run_stem(&c->holder, x_nchw, B, H, W, Hin, Win, (float*)workspace, out_nhwc, (cudaStream_t)stream);
+    return run_stem(mode, c->conv, x_nchw, B, H, W, Hin, Win, (float*)workspace, out_nhwc, (cudaStream_t)stream);
 }
 
 // conv3 + projection shortcut of a first bottleneck block as the f16x3 network runs them: one K-concatenated 1x1 conv (build_c3ds)
@@ -685,23 +630,23 @@ extern "C" int irn_shortcut_conv_create(const float* w3, const float* bn3, const
                                         int stride, irn_conv** out) {
     if (!w3 || !bn3 || !wds || !bnds || !out || planes <= 0 || cin <= 0 || !(stride == 1 || stride == 2))
         return fail(kBadArg, "irn_shortcut_conv_create: bad argument");
-    if (planes % kBfBK != 0 || cin % kBfBK != 0)
+    if (!c3ds_eligible(planes, cin, stride))
         return fail(kUnsupported, "irn_shortcut_conv_create: the fused conv needs planes %% %d == 0 and cin %% %d == 0 (got %d, %d)", kBfBK,
                     kBfBK, planes, cin);
     const int cout = planes * 4;
     std::vector<float> b3(w3, w3 + (size_t)cout * planes), bd(wds, wds + (size_t)cout * cin);
     b3.insert(b3.end(), bn3, bn3 + 4 * (size_t)cout);
     bd.insert(bd.end(), bnds, bnds + 4 * (size_t)cout);
-    irn_conv* c = new irn_conv();
-    Block& blk = c->holder.blocks[0].emplace_back();
+    irn_conv* c = new irn_conv(irn_conv::kShortcut);
+    Block& blk = c->block;
     Reader r3{b3.data(), b3.size()}, rd{bd.data(), bd.size()};
-    int rc = read_conv(&c->holder, r3, blk.c3, planes, cout, 1, 1, 0, true);
-    if (!rc) rc = read_conv(&c->holder, rd, blk.ds, cin, cout, 1, stride, 0, true);
+    HostWeights h3, hds;
+    int rc = read_conv(c->mem, r3, blk.c3, planes, cout, 1, 1, 0, true, &h3);
+    if (!rc) rc = read_conv(c->mem, rd, blk.ds, cin, cout, 1, stride, 0, true, &hds);
     blk.has_ds = true;
-    if (!rc) rc = build_c3ds(&c->holder, blk, cin, planes);
-    if (!rc && !blk.has_c3ds) rc = fail(kUnsupported, "irn_shortcut_conv_create: the fused conv is not eligible for the f16x3 kernel");
+    if (!rc) rc = build_c3ds(c->mem, blk, h3, hds);
     if (rc) {
-        irn_conv_destroy(c);
+        delete c;
         return rc;
     }
     *out = c;
@@ -711,9 +656,9 @@ extern "C" int irn_shortcut_conv_create(const float* w3, const float* bn3, const
 // relu(conv3(t2) + shortcut(x)): x NHWC [B,H,W,cin], t2 and out NHWC on the strided grid [B,Ho,Wo,planes | 4 planes]
 extern "C" int irn_shortcut_conv_forward(irn_conv* c, const float* t2, const float* x, int B, int H, int W, float* out, irn_stream_t stream) {
     launch_counter() = 0;
-    if (!c || c->holder.blocks[0].size() != 1 || !t2 || !x || !out || B <= 0 || H <= 0 || W <= 0)
-        return fail(kBadArg, "irn_shortcut_conv_forward: bad argument");
-    const Block& blk = c->holder.blocks[0][0];
+    if (!c || c->kind != irn_conv::kShortcut) return fail(kBadArg, "irn_shortcut_conv_forward: not a handle from irn_shortcut_conv_create");
+    if (!t2 || !x || !out || B <= 0 || H <= 0 || W <= 0) return fail(kBadArg, "irn_shortcut_conv_forward: bad argument");
+    const Block& blk = c->block;
     return run_c3ds(blk, t2, x, B, H, W, conv_out(H, 1, blk.ds.stride, 0), conv_out(W, 1, blk.ds.stride, 0), out, (cudaStream_t)stream);
 }
 
@@ -721,12 +666,15 @@ extern "C" int irn_shortcut_conv_forward(irn_conv* c, const float* t2, const flo
 extern "C" int irn_conv_forward(irn_conv* c, const float* in, int B, int H, int W, const float* residual, float* out, int relu, int mode,
                                 irn_stream_t stream) {
     launch_counter() = 0;
-    if (!c || !in || !out || B <= 0 || H <= 0 || W <= 0) return fail(kBadArg, "irn_conv_forward: bad argument");
+    if (!c || c->kind != irn_conv::kConv) return fail(kBadArg, "irn_conv_forward: not a handle from irn_conv_create");
+    if (!in || !out || B <= 0 || H <= 0 || W <= 0) return fail(kBadArg, "irn_conv_forward: bad argument");
     if (mode < 0 || mode > 2) return fail(kBadArg, "irn_conv_forward: mode must be 0, 1 or 2");
-    if (mode == 1 && c->conv.bn == 0) return fail(kUnsupported, "irn_conv_forward: this convolution is not eligible for the tensor-core kernel (Cin %% 32, Cout %% 64, k in {1,3}, stride in {1,2})");
-    if (mode == 2 && !c->conv.bf_ok) return fail(kUnsupported, "irn_conv_forward: this convolution is not eligible for the f16x3 kernel (Cin %% 64, Cout %% 64, k in {1,3}, stride in {1,2})");
-    c->holder.conv_mode = mode;
-    return run_conv(&c->holder, c->conv, in, B, H, W, residual, out, relu != 0, (cudaStream_t)stream, nullptr, nullptr);
+    const Conv& cv = c->conv;
+    const int bk = mode == 2 ? kBfBK : kTcBK;
+    if (mode >= 1 && !split_eligible(cv.cin, cv.cout, cv.k, cv.stride, bk))
+        return fail(kUnsupported, "irn_conv_forward: this convolution is not eligible for the %s kernel (Cin %% %d, Cout %% 64, k in {1,3}, stride in {1,2})",
+                    mode == 2 ? "f16x3" : "3xTF32", bk);
+    return run_conv(mode, cv, in, B, H, W, residual, out, relu != 0, (cudaStream_t)stream, nullptr, nullptr);
 }
 
 extern "C" int irn_net_set_conv_mode(irn_net* net, int mode) {
@@ -737,11 +685,7 @@ extern "C" int irn_net_set_conv_mode(irn_net* net, int mode) {
 
 extern "C" int irn_net_get_conv_mode(const irn_net* net) { return net ? net->conv_mode : -1; }
 
-extern "C" void irn_net_destroy(irn_net* net) {
-    if (!net) return;
-    for (void* p : net->allocs) cudaFree(p);
-    delete net;
-}
+extern "C" void irn_net_destroy(irn_net* net) { delete net; }
 
 extern "C" int irn_cam_net_create(const float* params, size_t n_floats, irn_net** out) {
     if (!params || !out) return fail(kBadArg, "irn_cam_net_create: null pointer");
@@ -751,12 +695,12 @@ extern "C" int irn_cam_net_create(const float* params, size_t n_floats, irn_net*
     int rc = read_trunk(net, rd);
     if (!rc) {
         const float* cw = rd.p;
-        rc = read_vec(net, rd, (size_t)20 * 2048, &net->classifier);
+        rc = read_vec(net->mem, rd, (size_t)20 * 2048, &net->classifier);
         if (!rc) {
             std::vector<float> padded((size_t)64 * 2048, 0.f);
             std::memcpy(padded.data(), cw, (size_t)20 * 2048 * sizeof(float));
             Reader r2{padded.data(), padded.size()};
-            rc = read_conv(net, r2, net->cls_conv, 2048, 64, 1, 1, 0, false);
+            rc = read_conv(net->mem, r2, net->cls_conv, 2048, 64, 1, 1, 0, false);
         }
     }
     if (!rc && rd.left != 0) rc = fail(kBadArg, "irn_cam_net_create: %zu unread floats in the parameter blob", rd.left);
@@ -776,14 +720,14 @@ extern "C" int irn_irn_net_create(const float* params, size_t n_floats, irn_net*
     int rc = read_trunk(net, rd);
     // heads in the order of net/resnet50_irn.py:23-93
     static const int e_cin[5] = {64, 256, 512, 1024, 2048}, e_up[5] = {1, 1, 2, 4, 4};
-    for (int i = 0; i < 5 && !rc; ++i) rc = read_head(net, rd, net->edge[i], e_cin[i], 32, 4, e_up[i]);
-    if (!rc) rc = read_vec(net, rd, 160, &net->edge6_w);
-    if (!rc) rc = read_vec(net, rd, 1, &net->edge6_b);
+    for (int i = 0; i < 5 && !rc; ++i) rc = read_head(net->mem, rd, net->edge[i], e_cin[i], 32, 4, e_up[i]);
+    if (!rc) rc = read_vec(net->mem, rd, 160, &net->edge6_w);
+    if (!rc) rc = read_vec(net->mem, rd, 1, &net->edge6_b);
     static const int d_cin[7] = {64, 256, 512, 1024, 2048, 768, 448}, d_cout[7] = {64, 128, 256, 256, 256, 256, 256},
                      d_g[7] = {8, 16, 16, 16, 16, 16, 16}, d_up[7] = {1, 1, 1, 2, 2, 2, 1};
-    for (int i = 0; i < 7 && !rc; ++i) rc = read_head(net, rd, net->dp[i], d_cin[i], d_cout[i], d_g[i], d_up[i]);
-    if (!rc) rc = read_vec(net, rd, 2 * 256, &net->dp7_w);
-    if (!rc) rc = read_vec(net, rd, 2, &net->mean_shift);
+    for (int i = 0; i < 7 && !rc; ++i) rc = read_head(net->mem, rd, net->dp[i], d_cin[i], d_cout[i], d_g[i], d_up[i]);
+    if (!rc) rc = read_vec(net->mem, rd, 2 * 256, &net->dp7_w);
+    if (!rc) rc = read_vec(net->mem, rd, 2, &net->mean_shift);
     if (!rc && rd.left != 0) rc = fail(kBadArg, "irn_irn_net_create: %zu unread floats in the parameter blob", rd.left);
     if (rc) {
         irn_net_destroy(net);
@@ -813,12 +757,12 @@ extern "C" int irn_cam_forward(const irn_net* net, const float* x_nchw, int B, i
     int rc = run_trunk(net, x_nchw, B, H, W, H, W, ar, false, feats, sh, st);
     if (rc) return rc;
     const int P = B / 2, h = sh.Hl[3], w = sh.Wl[3];
-    if (net->conv_mode >= 1 && net->cls_conv.bn) {
+    if (net->conv_mode >= 1 && net->cls_conv.tf32.ok) {
         // classifier as a 2048 -> 64 tensor-core conv with fused ReLU (the one-warp-per-pixel head re-reads the 160 KB weight
         // matrix per pixel), then flip-add + NHWC -> NCHW on the 20 real channels
         float* tmp = ar.take((size_t)B * h * w * 64);
         if (!ar.ok) return fail(kWorkspace, "irn_cam_forward: workspace too small");
-        if ((rc = run_conv(net, net->cls_conv, feats[4], B, h, w, nullptr, tmp, true, st, nullptr, nullptr))) return rc;
+        if ((rc = run_conv(net->conv_mode, net->cls_conv, feats[4], B, h, w, nullptr, tmp, true, st, nullptr, nullptr))) return rc;
         const size_t total = (size_t)P * 20 * h * w;
         cam_flip_add_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(tmp, cam_out, P, h, w, 64);
         IRN_LAUNCH_CHECK("cam_flip_add_kernel");
@@ -853,7 +797,7 @@ extern "C" size_t irn_edge_displacement_workspace_bytes(int P, int H, int W, int
 
 static int run_head(const irn_net* net, const Head& hd, const float* x, int B, int H, int W, float* raw, float* stats, float* dst, int Hd, int Wd, int Cd,
                     int coff, cudaStream_t st) {
-    int rc = run_conv(net, hd.conv, x, B, H, W, nullptr, raw, false, st, nullptr, nullptr);
+    int rc = run_conv(net->conv_mode, hd.conv, x, B, H, W, nullptr, raw, false, st, nullptr, nullptr);
     if (rc) return rc;
     if (hd.conv.cout > 256 || 256 % hd.conv.cout != 0 || hd.groups > 16) return fail(kUnsupported, "GroupNorm head with %d channels / %d groups", hd.conv.cout, hd.groups);
     IRN_CUDA(cudaMemsetAsync(stats, 0, (size_t)B * hd.groups * 2 * sizeof(double), st));

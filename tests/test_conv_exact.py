@@ -197,7 +197,7 @@ def tf32_split(a):
 
 
 def f16_weight_split(w):
-    """make_bf16_weights: per output channel, scale by 2^sh so that max |w| lies in [1, 2), then fp16 hi = rn(v),
+    """pack_split (f16x3): per output channel, scale by 2^sh so that max |w| lies in [1, 2), then fp16 hi = rn(v),
     lo = rn(v - hi).  Returns (v, hi, lo) in the scaled units."""
     flat = w.reshape(len(w), -1)
     v = np.empty_like(flat)
@@ -349,6 +349,33 @@ def test_shortcut_refuses_ineligible_shapes(built_lib):
     bn = [np.ones(128, np.float32), np.zeros(128, np.float32), np.zeros(128, np.float32), np.ones(128, np.float32)]
     with pytest.raises(_lib.IrnError, match="planes % 64"):
         ShortcutConv(np.zeros((128, 32), np.float32), bn, np.zeros((128, 64), np.float32), bn, 2)
+
+
+@pytest.mark.gpu
+def test_forward_refuses_another_kind_of_handle(cuda_dev):
+    """irn_conv_forward, irn_stem_forward and irn_shortcut_conv_forward each take only handles made by their own create call:
+    given one of the other two kinds they return kBadArg (-1) and launch nothing, in the default mode 2."""
+    from irn_b200 import _lib
+    from irn_b200.ops import Conv2d, ShortcutConv, Stem
+    bn = [np.ones(256, np.float32), np.zeros(256, np.float32), np.zeros(256, np.float32), np.ones(256, np.float32)]
+    ops = {"conv": Conv2d(np.zeros((64, 64, 1, 1), np.float32)), "stem": Stem(np.zeros((64, 3, 7, 7), np.float32)),
+           "shortcut": ShortcutConv(np.zeros((256, 64), np.float32), bn, np.zeros((256, 64), np.float32), bn, 1)}
+    L, st = _lib.lib(), _lib.stream_ptr()
+    buf = torch.zeros(1 << 20, device="cuda")   # holds every operand of a 1 x 16 x 16 call of any kind
+    p, ws = _lib.ptr(buf), L.irn_stem_workspace_bytes(1, 16, 16)
+    forward = {
+        "conv": lambda h: L.irn_conv_forward(h, p, 1, 16, 16, None, p, 1, 2, st),
+        "stem": lambda h: L.irn_stem_forward(h, p, 1, 16, 16, 16, 16, p, 2, p, ws, st),
+        "shortcut": lambda h: L.irn_shortcut_conv_forward(h, p, p, 1, 16, 16, p, st),
+    }
+    for call, run in forward.items():
+        for kind, op in ops.items():
+            if kind == call:
+                continue
+            launches = L.irn_total_launch_count()
+            rc = run(op._h)
+            assert rc == -1, "%s forward on a %s handle returned %d: %s" % (call, kind, rc, L.irn_last_error().decode())
+            assert L.irn_total_launch_count() == launches, "%s forward on a %s handle launched a kernel" % (call, kind)
 
 
 # ------------------------------------------------------------------------------------------------------------- GPU: real data

@@ -1,4 +1,4 @@
-"""CAM / EdgeDisplacement errors against the reference goldens for a conv mode (development aid; env switches of nets.cu apply).
+"""CAM / EdgeDisplacement errors against the reference goldens for a conv mode (development aid).
     python tools/net_err.py [mode=2]"""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
