@@ -91,10 +91,13 @@ int irn_random_walk(const float* x, const float* edge, float* out, int n_img,
                     int n_iter, void* workspace, size_t workspace_bytes, irn_stream_t stream);
 
 /* Same, selecting the kernel: variant 0 = production (radius 5: the fused cluster kernel -- all
- * n_iter steps in one launch, weights resident in shared memory -- when h, w <= 128, else the
- * per-step TMA kernel), 1 = generic bounds-checked step kernel (any radius 2..10; validation /
- * radii the reference's hot path never uses), 2 = per-step TMA kernel (radius 5), 3 = persistent
- * TMA-ring step kernel (experiment), 4 = fused cluster kernel, or -4 when it cannot run. */
+ * n_iter steps in one launch, weights resident in shared memory -- or the per-step TMA kernel,
+ * whichever a cost model expects to be faster; the fused kernel needs h, w <= 128; other radii:
+ * the generic kernel), 1 = generic bounds-checked step kernel (any radius 2..10; validation /
+ * radii the reference's hot path never uses), 2 = per-step TMA kernel (radius 5), 4 = fused
+ * cluster kernel.  Variants 2 and 4 return -4 when they cannot run as asked; any other variant
+ * returns -1.  Both are reported before anything is launched (except a device that cannot
+ * co-schedule variant 4's cluster, which is found at launch time). */
 int irn_random_walk_variant(const float* x, const float* edge, float* out, int n_img,
                             const int32_t* chan_offsets, int h, int w, int radius, double beta,
                             int n_iter, void* workspace, size_t workspace_bytes, int variant,

@@ -278,10 +278,7 @@ __device__ __forceinline__ void static_for(F&& f) {
 
 constexpr int kR = 4;                 // stencil reach for radius 5
 constexpr int kTX = 32;               // tile width = one warp
-#ifndef IRN_RW_PY
-#define IRN_RW_PY 4
-#endif
-constexpr int kPY = IRN_RW_PY;        // rows per thread (register window)
+constexpr int kPY = 4;                // rows per thread (register window), in the step and the fused kernel
 constexpr int kWarps = 4;
 constexpr int kTY = kPY * kWarps;     // 16
 constexpr int kSW = kTX + 2 * kR;     // 40 columns staged (x0-4 .. x0+35)
@@ -298,6 +295,57 @@ __device__ __forceinline__ double widen_weight(float f) {
     return __hiloint2double((int)((u >> 3) + 0x38000000u), (int)(u << 29));
 }
 
+// One tap of the radius-5 stencil, all compile-time: |dx| class, column offset dxc of the state value, window row r (relative
+// to the thread's first row), output row j and the internal weight plane k the tap reads.
+template <int CLS, int DXC, int R, int J, int K>
+struct Tap5 {
+    static constexpr int cls = CLS, dxc = DXC, r = R, j = J, k = K;
+};
+
+struct NoHook {
+    template <class T>
+    __device__ __forceinline__ void operator()(T) const {}
+};
+
+// The 69-tap update of PY consecutive rows x NC channels of one column, accumulated into acc (which holds the diagonal term).
+// For every column offset dxc and window row r the state value y(r, dxc, c) is read ONCE and used by every (row j, tap) pair
+// it takes part in:
+//   forward tap  d = (r-j, dxc):   weight W_d(p_j)                        w_fwd(Tap5)
+//   mirrored tap d = (j-r, -dxc):  weight W_d(p_j - d) = W_d at the cell being read   w_mir(Tap5)
+// Taps are applied in one fixed order -- class 0..4, sign + then -, r = -kR .. PY+kR-1, j = 0..PY-1, forward before mirrored
+// -- so every kernel that walks through this helper produces bit-identical results.  enter(CLS) / leave(CLS) run around each
+// |dx| class (the step kernel waits for and refills its weight buffers there).
+template <int PY, int NC, class YRead, class WFwd, class WMir, class Enter = NoHook, class Leave = NoHook>
+__device__ __forceinline__ void stencil69(double (&acc)[PY][NC], YRead&& y, WFwd&& w_fwd, WMir&& w_mir, Enter&& enter = Enter{},
+                                          Leave&& leave = Leave{}) {
+    static_for<0, 5>([&](auto CLS) {
+        constexpr int cls = decltype(CLS)::value;
+        enter(CLS);
+        static_for<0, (cls == 0 ? 1 : 2)>([&](auto SGN) {
+            constexpr int dxc = decltype(SGN)::value == 0 ? cls : -cls;
+            static_for<-kR, PY + kR>([&](auto RR) {
+                constexpr int r = decltype(RR)::value;
+                double v[NC];   // static_for, not #pragma unroll: a one-trip loop (NC = 1) made the fused kernel ~3 % slower
+                static_for<0, NC>([&](auto C) { v[C] = y(r, dxc, C); });
+                static_for<0, PY>([&](auto JJ) {
+                    constexpr int j = decltype(JJ)::value;
+                    constexpr int dy = r - j;
+                    constexpr int kf = plane5(dy, dxc);
+                    constexpr int kb = plane5(-dy, -dxc);
+                    if constexpr (kf >= 0) {
+                        const double wv = widen_weight(w_fwd(Tap5<cls, dxc, r, j, kf>{}));
+                        static_for<0, NC>([&](auto C) { acc[j][C] = fma(wv, v[C], acc[j][C]); });
+                    } else if constexpr (kb >= 0) {
+                        const double wv = widen_weight(w_mir(Tap5<cls, dxc, r, j, kb>{}));
+                        static_for<0, NC>([&](auto C) { acc[j][C] = fma(wv, v[C], acc[j][C]); });
+                    }
+                });
+            });
+        });
+        leave(CLS);
+    });
+}
+
 constexpr size_t rw_tma_smem_bytes(int ch) {
     return 128 /*alignment slack*/ + (size_t)ch * kYH * kSW * sizeof(double) + 2 * (size_t)kWBufFloats * sizeof(float) + 64;
 }
@@ -307,17 +355,13 @@ struct RwMaps {
     CUtensorMap y[4];   // state being read, box depth 1..4 channels
 };
 
-// One walk step for CH channels of one 32x16 tile.  Thread = one column, kPY consecutive rows.
-// For every column offset dxc and window row r the state value y(yb+r, x+dxc) is read from shared
-// memory ONCE and used by every (row j, tap) pair it participates in:
-//   forward tap  d=(r-j, dxc):   weight W_d(p_j)                      (own cell of plane d)
-//   mirrored tap d=(j-r,-dxc):   weight W_d(p_j - d) = W_d at the very cell being read
+// One walk step for CH channels of one 32x16 tile.  Thread = one column, kPY consecutive rows; state tile in shared memory.
 // The 34 weight planes stream through two shared-memory buffers one |dx| class at a time (TMA,
 // zero-filled outside the image, which is exactly the reference's "affinity 0 to anything outside").
 // One channel chunk (CH = 1..4 channels of one image) of one tile: issue the TMA loads, run the five |dx| classes, store.
 template <int CH>
 __device__ __forceinline__ void rw_chunk(const RwMaps& maps, const double* __restrict__ inv_s, double* __restrict__ yout, double* s_y,
-                                         float* s_w, uint64_t* bars, uint32_t& ph_y, uint32_t& ph_w0, uint32_t& ph_w1, int img, int c0,
+                                         float* s_w, uint64_t* bars, uint32_t& ph_y, uint32_t (&ph_w)[2], int img, int c0,
                                          int c_end, int x0, int y0, int h, int w, int pitch) {
     const int tid = threadIdx.x;
     const int lane = tid & 31, warp = tid >> 5;
@@ -343,50 +387,34 @@ __device__ __forceinline__ void rw_chunk(const RwMaps& maps, const double* __res
 #pragma unroll
             for (int c = 0; c < CH; ++c) acc[j][c] = s_y[(c * kYH + ty0 + j + kR) * kSW + lane + kR];   // diagonal weight 1
 
-        static_for<0, 5>([&](auto CLS) {
-            constexpr int cls = decltype(CLS)::value;
-            constexpr int buf = cls & 1;
-            const float* wb = s_w + buf * kWBufFloats;
-            if constexpr (buf == 0) {
-                mbar_wait(&bars[1], ph_w0);
-                ph_w0 ^= 1;
-            } else {
-                mbar_wait(&bars[2], ph_w1);
-                ph_w1 ^= 1;
-            }
-            static_for<0, (cls == 0 ? 1 : 2)>([&](auto SGN) {
-                constexpr int dxc = decltype(SGN)::value == 0 ? cls : -cls;
-                static_for<-kR, kPY + kR>([&](auto RR) {
-                    constexpr int r = decltype(RR)::value;
-                    double v[CH];
-#pragma unroll
-                    for (int c = 0; c < CH; ++c) v[c] = s_y[(c * kYH + ty0 + r + kR) * kSW + lane + dxc + kR];
-                    static_for<0, kPY>([&](auto JJ) {
-                        constexpr int j = decltype(JJ)::value;
-                        constexpr int dy = r - j;
-                        constexpr int kf = plane5(dy, dxc);
-                        constexpr int kb = plane5(-dy, -dxc);
-                        if constexpr (kf >= 0) {
-                            const double wv = widen_weight(wb[((kf - cls_base5(cls)) * kWH + ty0 + j + kR) * kSW + lane + kR]);
-#pragma unroll
-                            for (int c = 0; c < CH; ++c) acc[j][c] = fma(wv, v[c], acc[j][c]);
-                        } else if constexpr (kb >= 0) {
-                            const double wv = widen_weight(wb[((kb - cls_base5(cls)) * kWH + ty0 + r + kR) * kSW + lane + dxc + kR]);
-#pragma unroll
-                            for (int c = 0; c < CH; ++c) acc[j][c] = fma(wv, v[c], acc[j][c]);
-                        }
-                    });
-                });
-            });
-            if constexpr (cls + 2 <= 4) {
-                __syncthreads();   // every thread is done reading buffer `buf`
-                if (tid == 0) {
-                    uint64_t* bar = &bars[1 + buf];
-                    mbar_arrive_expect_tx(bar, (uint32_t)((cls_base5(cls + 3) - cls_base5(cls + 2)) * kWH * kSW * sizeof(float)));
-                    tma_load_3d(s_w + buf * kWBufFloats, &maps.w[cls + 2], bar, x0 - kR, y0 - kR, img * 34 + cls_base5(cls + 2));
+        stencil69(
+            acc, [&](int r, int dxc, int c) { return s_y[(c * kYH + ty0 + r + kR) * kSW + lane + dxc + kR]; },
+            [&](auto t) {   // buffer cls & 1 holds the planes of class cls
+                using T = decltype(t);
+                const float* wb = s_w + (T::cls & 1) * kWBufFloats;
+                return wb[((T::k - cls_base5(T::cls)) * kWH + ty0 + T::j + kR) * kSW + lane + kR];
+            },
+            [&](auto t) {
+                using T = decltype(t);
+                const float* wb = s_w + (T::cls & 1) * kWBufFloats;
+                return wb[((T::k - cls_base5(T::cls)) * kWH + ty0 + T::r + kR) * kSW + lane + T::dxc + kR];
+            },
+            [&](auto CLS) {
+                constexpr int buf = decltype(CLS)::value & 1;
+                mbar_wait(&bars[1 + buf], ph_w[buf]);
+                ph_w[buf] ^= 1;
+            },
+            [&](auto CLS) {
+                constexpr int cls = decltype(CLS)::value, buf = cls & 1;
+                if constexpr (cls + 2 <= 4) {
+                    __syncthreads();   // every thread is done reading buffer `buf`: refill it with class cls + 2
+                    if (tid == 0) {
+                        uint64_t* bar = &bars[1 + buf];
+                        mbar_arrive_expect_tx(bar, (uint32_t)((cls_base5(cls + 3) - cls_base5(cls + 2)) * kWH * kSW * sizeof(float)));
+                        tma_load_3d(s_w + buf * kWBufFloats, &maps.w[cls + 2], bar, x0 - kR, y0 - kR, img * 34 + cls_base5(cls + 2));
+                    }
                 }
-            }
-        });
+            });
 
         if (x < w) {
 #pragma unroll
@@ -426,165 +454,18 @@ rw_step_tma_kernel(const __grid_constant__ RwMaps maps, const double* __restrict
         fence_mbar_init();
     }
     __syncthreads();
-    uint32_t ph_y = 0, ph_w0 = 0, ph_w1 = 0;
+    uint32_t ph_y = 0, ph_w[2] = {0, 0};
     int c0 = c_begin;
     while (c0 < c_end) {
         const int n = c_end - c0 < MAXCH ? c_end - c0 : MAXCH;
-        if (MAXCH >= 4 && n == 4) rw_chunk<4>(maps, inv_s, yout, s_y, s_w, bars, ph_y, ph_w0, ph_w1, img, c0, c_end, x0, y0, h, w, pitch);
-        else if (MAXCH >= 3 && n == 3) rw_chunk<3>(maps, inv_s, yout, s_y, s_w, bars, ph_y, ph_w0, ph_w1, img, c0, c_end, x0, y0, h, w, pitch);
-        else if (MAXCH >= 2 && n == 2) rw_chunk<2>(maps, inv_s, yout, s_y, s_w, bars, ph_y, ph_w0, ph_w1, img, c0, c_end, x0, y0, h, w, pitch);
-        else rw_chunk<1>(maps, inv_s, yout, s_y, s_w, bars, ph_y, ph_w0, ph_w1, img, c0, c_end, x0, y0, h, w, pitch);
+        if (MAXCH >= 4 && n == 4) rw_chunk<4>(maps, inv_s, yout, s_y, s_w, bars, ph_y, ph_w, img, c0, c_end, x0, y0, h, w, pitch);
+        else if (MAXCH >= 3 && n == 3) rw_chunk<3>(maps, inv_s, yout, s_y, s_w, bars, ph_y, ph_w, img, c0, c_end, x0, y0, h, w, pitch);
+        else if (MAXCH >= 2 && n == 2) rw_chunk<2>(maps, inv_s, yout, s_y, s_w, bars, ph_y, ph_w, img, c0, c_end, x0, y0, h, w, pitch);
+        else rw_chunk<1>(maps, inv_s, yout, s_y, s_w, bars, ph_y, ph_w, img, c0, c_end, x0, y0, h, w, pitch);
         c0 += n;
         __syncthreads();   // s_y / weight buffers are reused by the next channel chunk
     }
 }
-
-#ifdef IRN_EXPERIMENTAL   // persistent ring variant of the per-step kernel: an experiment, not in the product build
-// ---------------------------------------------------------------- persistent ring step kernel (radius 5, experiment, variant 3)
-// Same arithmetic as rw_step_tma_kernel, restructured so that TMA latency is never exposed: one persistent CTA per SM
-// walks tiles b, b+G, b+2G, ...; warp 4 is a TMA producer that runs ahead through a ring of kRingW weight-class buffers and
-// two state-tile buffers (full/empty mbarriers, no __syncthreads in the loop), warps 0-3 consume.  ~200 KB of loads stay
-// in flight per SM instead of ~60 KB.
-template <int CH>
-struct RingCfg {
-    static constexpr int kYBytes = CH * kYH * kSW * (int)sizeof(double);
-    static constexpr int kWBytes = kWBufFloats * (int)sizeof(float);
-    static constexpr int kStagesW = (227 * 1024 - 2 * kYBytes - 512) / kWBytes > 8 ? 8 : (227 * 1024 - 2 * kYBytes - 512) / kWBytes;
-    static constexpr int kSmem = 2 * kYBytes + kStagesW * kWBytes + 512;
-};
-
-template <int CH>
-__global__ void __launch_bounds__(kTX* kWarps + 32, 1)
-rw_step_ring_kernel(const __grid_constant__ RwMaps maps, const double* __restrict__ inv_s, double* __restrict__ yout,
-                    const int* __restrict__ chan_off, int h, int w, int pitch, int n_img, int tiles_x, int tiles_y) {
-    using Cfg = RingCfg<CH>;
-    constexpr int NW = Cfg::kStagesW;
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    double* s_y = (double*)smem_raw;                                   // [2][CH][kYH][kSW]
-    float* s_w = (float*)(smem_raw + 2 * Cfg::kYBytes);               // [NW][<=9][kWH][kSW]
-    uint64_t* bars = (uint64_t*)(smem_raw + 2 * Cfg::kYBytes + NW * Cfg::kWBytes);
-    uint64_t* fullY = bars;            // [2]
-    uint64_t* emptyY = bars + 2;       // [2]
-    uint64_t* fullW = bars + 4;        // [NW]
-    uint64_t* emptyW = bars + 4 + NW;  // [NW]
-
-    const int tid = threadIdx.x;
-    const int warp = tid >> 5, lane = tid & 31;
-    if (tid == 0) {
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&fullY[i], 1);
-            mbar_init(&emptyY[i], kWarps);
-        }
-        for (int i = 0; i < NW; ++i) {
-            mbar_init(&fullW[i], 1);
-            mbar_init(&emptyW[i], kWarps);
-        }
-        fence_mbar_init();
-    }
-    __syncthreads();
-
-    const int tiles = tiles_x * tiles_y;
-    const int n_items = n_img * tiles;
-    const size_t plane_sz = (size_t)h * pitch;
-
-    if (warp == kWarps) {
-        // ------------------------------------------------ producer
-        if (lane == 0) {
-            uint32_t ny = 0, nw = 0;   // sub-items / weight chunks issued so far
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                const int img = item / tiles, t = item % tiles;
-                const int x0 = (t % tiles_x) * kTX, y0 = (t / tiles_x) * kTY;
-                const int c_begin = chan_off[img], c_end = chan_off[img + 1];
-                for (int c0 = c_begin; c0 < c_end; c0 += CH) {
-                    const uint32_t ys = ny & 1;
-                    mbar_wait(&emptyY[ys], ((ny >> 1) & 1) ^ 1);
-                    mbar_arrive_expect_tx(&fullY[ys], (uint32_t)Cfg::kYBytes);
-                    tma_load_3d((unsigned char*)s_y + ys * Cfg::kYBytes, &maps.y[CH - 1], &fullY[ys], x0 - kR, y0 - kR, c0);
-                    ++ny;
-#pragma unroll
-                    for (int cls = 0; cls < 5; ++cls) {
-                        const uint32_t slot = nw % NW;
-                        mbar_wait(&emptyW[slot], ((nw / NW) & 1) ^ 1);
-                        mbar_arrive_expect_tx(&fullW[slot], (uint32_t)((cls_base5(cls + 1) - cls_base5(cls)) * kWH * kSW * sizeof(float)));
-                        tma_load_3d(s_w + slot * kWBufFloats, &maps.w[cls], &fullW[slot], x0 - kR, y0 - kR, img * 34 + cls_base5(cls));
-                        ++nw;
-                    }
-                }
-            }
-        }
-        return;
-    }
-
-    // ---------------------------------------------------- consumers (warps 0..3)
-    const int ty0 = warp * kPY;
-    uint32_t ny = 0, nw = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int img = item / tiles, t = item % tiles;
-        const int x0 = (t % tiles_x) * kTX, y0 = (t / tiles_x) * kTY;
-        const int x = x0 + lane, yb = y0 + ty0;
-        const int c_begin = chan_off[img], c_end = chan_off[img + 1];
-        for (int c0 = c_begin; c0 < c_end; c0 += CH) {
-            const uint32_t ys = ny & 1;
-            const double* sy = (const double*)((const unsigned char*)s_y + ys * Cfg::kYBytes);
-            mbar_wait(&fullY[ys], (ny >> 1) & 1);
-            ++ny;
-            double acc[kPY][CH];
-#pragma unroll
-            for (int j = 0; j < kPY; ++j)
-#pragma unroll
-                for (int c = 0; c < CH; ++c) acc[j][c] = sy[(c * kYH + ty0 + j + kR) * kSW + lane + kR];   // diagonal weight 1
-
-            static_for<0, 5>([&](auto CLS) {
-                constexpr int cls = decltype(CLS)::value;
-                const uint32_t slot = nw % NW;
-                const float* wb = s_w + slot * kWBufFloats;
-                mbar_wait(&fullW[slot], (nw / NW) & 1);
-                ++nw;
-                static_for<0, (cls == 0 ? 1 : 2)>([&](auto SGN) {
-                    constexpr int dxc = decltype(SGN)::value == 0 ? cls : -cls;
-                    static_for<-kR, kPY + kR>([&](auto RR) {
-                        constexpr int r = decltype(RR)::value;
-                        double v[CH];
-#pragma unroll
-                        for (int c = 0; c < CH; ++c) v[c] = sy[(c * kYH + ty0 + r + kR) * kSW + lane + dxc + kR];
-                        static_for<0, kPY>([&](auto JJ) {
-                            constexpr int j = decltype(JJ)::value;
-                            constexpr int dy = r - j;
-                            constexpr int kf = plane5(dy, dxc);
-                            constexpr int kb = plane5(-dy, -dxc);
-                            if constexpr (kf >= 0) {
-                                const double wv = widen_weight(wb[((kf - cls_base5(cls)) * kWH + ty0 + j + kR) * kSW + lane + kR]);
-#pragma unroll
-                                for (int c = 0; c < CH; ++c) acc[j][c] = fma(wv, v[c], acc[j][c]);
-                            } else if constexpr (kb >= 0) {
-                                const double wv = widen_weight(wb[((kb - cls_base5(cls)) * kWH + ty0 + r + kR) * kSW + lane + dxc + kR]);
-#pragma unroll
-                                for (int c = 0; c < CH; ++c) acc[j][c] = fma(wv, v[c], acc[j][c]);
-                            }
-                        });
-                    });
-                });
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&emptyW[slot]);   // this warp is done with the weight buffer
-            });
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&emptyY[ys]);          // ... and with the state tile
-
-            if (x < w) {
-#pragma unroll
-                for (int j = 0; j < kPY; ++j) {
-                    if (yb + j < h) {
-                        const double is = inv_s[(size_t)img * plane_sz + (size_t)(yb + j) * pitch + x];
-#pragma unroll
-                        for (int c = 0; c < CH; ++c)
-                            if (c0 + c < c_end) yout[(size_t)(c0 + c) * plane_sz + (size_t)(yb + j) * pitch + x] = acc[j][c] * is;
-                    }
-                }
-            }
-        }
-    }
-}
-#endif  // IRN_EXPERIMENTAL
 
 // ---------------------------------------------------------------- fused walk (radius 5, h,w <= 128): the production path
 // All n_iter steps of one (image, channel) in ONE launch, one thread-block cluster per item:
@@ -596,18 +477,12 @@ rw_step_ring_kernel(const __grid_constant__ RwMaps maps, const double* __restric
 //     either side); each step writes the new rows locally and pushes the boundary rows into the neighbour CTAs' halo rows
 //     through distributed shared memory, then ONE cluster barrier publishes them;
 //   * HBM traffic per item = weights + 1/s + seeds in, fp32 result out; nothing per step.
-// The tap order per pixel is the step kernel's, so both produce bit-identical results.
 constexpr int kFR = 8;                       // rows per CTA
 constexpr int kFW = 128;                     // widest supported grid = weight row pitch in shared memory
 constexpr int kFYP = kFW + 2 * kR;           // 136: state row pitch
 constexpr int kFYR = kFR + 2 * kR;           // 16 state rows
-#ifndef IRN_RW_REGPLANES4
-#define IRN_RW_REGPLANES4 16
-#endif
-#ifndef IRN_RW_REGPLANES2
-#define IRN_RW_REGPLANES2 16
-#endif
-constexpr int fused_threads(int py) { return (kFW / 32) * (kFR / py) * 32; }   // py = rows per thread: 4 -> 256, 2 -> 512 threads
+constexpr int kFThreads = (kFW / 32) * (kFR / kPY) * 32;   // 256: one column and kPY rows per thread
+constexpr int kFRegPlanes = 16;              // planes whose forward-tap weights live in registers
 
 __host__ __device__ constexpr int plane_dy5(int k) {   // dy of internal plane k (inverse of plane5)
     if (k < 4) return k + 1;
@@ -651,12 +526,10 @@ __device__ __forceinline__ void st_cluster_f64(uint32_t addr, double v) {
     asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(addr), "d"(v) : "memory");
 }
 
-template <int kFPY>
-__global__ void __launch_bounds__(fused_threads(kFPY), 1)
+__global__ void __launch_bounds__(kFThreads, 1)
 rw_fused_kernel(const float* __restrict__ W, const double* __restrict__ inv_s, const float* __restrict__ x,
                 const float* __restrict__ edge, float* __restrict__ out, const int* __restrict__ chan_off, int totc, int h, int w,
                 int pitch, int n_iter) {
-    constexpr int kFThreads = fused_threads(kFPY);
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float* s_w = (float*)(smem_raw + 16);
     double* s_y = (double*)(smem_raw + kFusedWBytes);   // [2][kFYR][kFYP]
@@ -669,7 +542,7 @@ rw_fused_kernel(const float* __restrict__ W, const double* __restrict__ inv_s, c
     const int r0 = rank * kFR;
     const bool active = r0 < h;            // CTAs below the image only take part in the barriers
     const int col = (warp & 3) * 32 + lane;
-    const int ty0 = (warp >> 2) * kFPY;
+    const int ty0 = (warp >> 2) * kPY;
     const size_t plane_sz = (size_t)h * pitch;
     const size_t hw = (size_t)h * w;
 
@@ -687,12 +560,11 @@ rw_fused_kernel(const float* __restrict__ W, const double* __restrict__ inv_s, c
     const uint32_t dn_addr = rank + 1 < csize ? cluster_map(sy_addr, (uint32_t)(rank + 1)) : 0u;
 
     int cur_img = -1;
-    constexpr int kRegPlanes = kFPY == 4 ? IRN_RW_REGPLANES4 : IRN_RW_REGPLANES2;   // planes whose forward weights live in registers
-    float wf[kFPY][kRegPlanes > 0 ? kRegPlanes : 1];
+    float wf[kPY][kFRegPlanes];
     for (int c = c_lo; c < c_hi; ++c) {
         int img = 0;
         while (chan_off[img + 1] <= c) ++img;
-        double val[kFPY], is[kFPY];
+        double val[kPY], is[kPY];
         if (active) {
             if (img != cur_img) {          // (the last step's barrier ordered every read of the previous weights before this)
                 const float* Wi = W + (size_t)img * 34 * plane_sz;
@@ -718,14 +590,14 @@ rw_fused_kernel(const float* __restrict__ W, const double* __restrict__ inv_s, c
             }
             if (img != cur_img) {          // forward-tap weights of this thread's pixels stay in registers for the whole walk:
                 __syncthreads();           // shared memory then serves only the mirrored taps (half of the weight reads)
-                static_for<0, kRegPlanes>([&](auto K) {
+                static_for<0, kFRegPlanes>([&](auto K) {
                     constexpr int k = decltype(K)::value;
 #pragma unroll
-                    for (int j = 0; j < kFPY; ++j) wf[j][k] = s_w[(wrow_base5(k) + plane_dy5(k) + ty0 + j) * kFW + col];
+                    for (int j = 0; j < kPY; ++j) wf[j][k] = s_w[(wrow_base5(k) + plane_dy5(k) + ty0 + j) * kFW + col];
                 });
             }
 #pragma unroll
-            for (int j = 0; j < kFPY; ++j) {
+            for (int j = 0; j < kPY; ++j) {
                 const int gr = r0 + ty0 + j;
                 const bool in = gr < h && col < w;
                 is[j] = in ? inv_s[(size_t)img * plane_sz + (size_t)gr * pitch + col] : 0.0;
@@ -741,7 +613,7 @@ rw_fused_kernel(const float* __restrict__ W, const double* __restrict__ inv_s, c
                 const uint32_t boff = (uint32_t)((t & 1) * kFYR * kFYP * sizeof(double));
                 double* sn = s_y + (t & 1) * kFYR * kFYP;
 #pragma unroll
-                for (int j = 0; j < kFPY; ++j) {
+                for (int j = 0; j < kPY; ++j) {
                     const int lr = ty0 + j;
                     sn[(kR + lr) * kFYP + kR + col] = val[j];
                     if (lr < kR) {
@@ -756,38 +628,27 @@ rw_fused_kernel(const float* __restrict__ W, const double* __restrict__ inv_s, c
             if (t == n_iter) break;
             if (active) {
                 const double* sy = s_y + (t & 1) * kFYR * kFYP;
-                double acc[kFPY];
+                double acc[kPY][1];
 #pragma unroll
-                for (int j = 0; j < kFPY; ++j) acc[j] = val[j];   // diagonal weight 1
-                static_for<0, 5>([&](auto CLS) {
-                    constexpr int cls = decltype(CLS)::value;
-                    static_for<0, (cls == 0 ? 1 : 2)>([&](auto SGN) {
-                        constexpr int dxc = decltype(SGN)::value == 0 ? cls : -cls;
-                        static_for<-kR, kFPY + kR>([&](auto RR) {
-                            constexpr int r = decltype(RR)::value;
-                            const double v = sy[(kR + ty0 + r) * kFYP + kR + col + dxc];
-                            static_for<0, kFPY>([&](auto JJ) {
-                                constexpr int j = decltype(JJ)::value;
-                                constexpr int dy = r - j;
-                                constexpr int kf = plane5(dy, dxc);
-                                constexpr int kb = plane5(-dy, -dxc);
-                                if constexpr (kf >= 0) {          // forward tap: W_kf at the pixel itself (register copy)
-                                    if constexpr (kf < kRegPlanes) acc[j] = fma(widen_weight(wf[j][kf]), v, acc[j]);
-                                    else acc[j] = fma(widen_weight(s_w[(wrow_base5(kf) + dy + ty0 + j) * kFW + col]), v, acc[j]);
-                                } else if constexpr (kb >= 0) {   // mirrored tap: W_kb at the pixel being read, (row ty0+r, col+dxc)
-                                    acc[j] = fma(widen_weight(s_w[(wrow_base5(kb) + ty0 + j) * kFW + col + dxc]), v, acc[j]);
-                                }
-                            });
-                        });
+                for (int j = 0; j < kPY; ++j) acc[j][0] = val[j];   // diagonal weight 1
+                stencil69(
+                    acc, [&](int r, int dxc, int) { return sy[(kR + ty0 + r) * kFYP + kR + col + dxc]; },
+                    [&](auto t) {   // W_k at the pixel itself: the register copy, or plane k's row (own row + dy)
+                        using T = decltype(t);
+                        if constexpr (T::k < kFRegPlanes) return wf[T::j][T::k];
+                        else return s_w[(wrow_base5(T::k) + (T::r - T::j) + ty0 + T::j) * kFW + col];
+                    },
+                    [&](auto t) {   // W_k at the pixel being read, (row ty0+r, col+dxc): plane k stores it in row ty0+j
+                        using T = decltype(t);
+                        return s_w[(wrow_base5(T::k) + ty0 + T::j) * kFW + col + T::dxc];
                     });
-                });
 #pragma unroll
-                for (int j = 0; j < kFPY; ++j) val[j] = acc[j] * is[j];
+                for (int j = 0; j < kPY; ++j) val[j] = acc[j][0] * is[j];
             }
         }
         if (active) {
 #pragma unroll
-            for (int j = 0; j < kFPY; ++j) {
+            for (int j = 0; j < kPY; ++j) {
                 const int gr = r0 + ty0 + j;
                 if (gr < h && col < w) out[(size_t)c * hw + (size_t)gr * w + col] = (float)val[j];
             }
@@ -826,8 +687,19 @@ static RwWorkspace carve(void* base, int n_img, int h, int w, int totc, int n_ds
     return ws;
 }
 
+template <int MODE>
+static int launch_affinity(const float* edge, float* out, int n_img, int h, int w, int pitch, int radius, double beta, int ibeta,
+                           cudaStream_t stream) {
+    const int R = radius - 1;
+    dim3 grid(((w + kAffTX - 1) / kAffTX) * ((h + kAffTY - 1) / kAffTY), n_img), block(kAffTX, kAffTY);
+    const size_t smem = (size_t)(kAffTY + R) * (kAffTX + 2 * R) * sizeof(float);
+    rw_affinity_kernel<MODE><<<grid, block, smem, stream>>>(edge, out, h, w, pitch, beta, ibeta);
+    IRN_LAUNCH_CHECK(MODE == 0 ? "rw_affinity_kernel<0>" : "rw_affinity_kernel<1>");
+    return kOk;
+}
+
 template <int CH>
-static int launch_tma_steps(const RwWorkspace& ws, int n_img, int totc, int h, int w, int n_iter, int variant, cudaStream_t stream) {
+static int launch_tma_steps(const RwWorkspace& ws, int n_img, int totc, int h, int w, int n_iter, cudaStream_t stream) {
     const int pitch = ws.pitch;
     RwMaps maps[2];
     for (int b = 0; b < 2; ++b) {
@@ -846,55 +718,41 @@ static int launch_tma_steps(const RwWorkspace& ws, int n_img, int totc, int h, i
             if (rc) return rc;
         }
     }
-    const int tiles_x = (w + kTX - 1) / kTX, tiles_y = (h + kTY - 1) / kTY;
-    if (variant != 3) {   // production: three 4-warp CTAs per SM, two weight buffers each (measured faster than the ring below for C >= 2)
-        const size_t smem = rw_tma_smem_bytes(CH);
+    // three 4-warp CTAs per SM, two weight buffers each (measured faster than a persistent one-CTA-per-SM TMA ring: 50 against
+    // 67 us/step at C = 2)
+    const size_t smem = rw_tma_smem_bytes(CH);
+    static DeviceOnce once;
+    const int ds = once.slot();
+    if (once.need(ds)) {
         IRN_CUDA(cudaFuncSetAttribute(rw_step_tma_kernel<CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        dim3 grid(tiles_x * tiles_y, n_img);
-        for (int it = 0; it < n_iter; ++it) {
-            rw_step_tma_kernel<CH><<<grid, kTX * kWarps, smem, stream>>>(maps[it & 1], ws.inv_s, ws.y[(it + 1) & 1], ws.chan_off, h, w, pitch);
-            IRN_LAUNCH_CHECK("rw_step_tma_kernel");
-        }
-        return kOk;
+        once.done[ds] = true;
     }
-#ifndef IRN_EXPERIMENTAL
-    return fail(kUnsupported, "irn_random_walk_variant: variant 3 (ring kernel) is an experiment, built only with -DIRN_EXPERIMENTAL");
-#else
-    int dev = 0, n_sm = 0;
-    IRN_CUDA(cudaGetDevice(&dev));
-    IRN_CUDA(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-    const int smem = RingCfg<CH>::kSmem;
-    IRN_CUDA(cudaFuncSetAttribute(rw_step_ring_kernel<CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    const int n_items = tiles_x * tiles_y * n_img;
-    const int grid = n_items < n_sm ? n_items : n_sm;   // one persistent CTA per SM
+    dim3 grid(((w + kTX - 1) / kTX) * ((h + kTY - 1) / kTY), n_img);
     for (int it = 0; it < n_iter; ++it) {
-        rw_step_ring_kernel<CH><<<grid, kTX * kWarps + 32, smem, stream>>>(maps[it & 1], ws.inv_s, ws.y[(it + 1) & 1], ws.chan_off, h, w, pitch,
-                                                                            n_img, tiles_x, tiles_y);
-        IRN_LAUNCH_CHECK("rw_step_ring_kernel");
+        rw_step_tma_kernel<CH><<<grid, kTX * kWarps, smem, stream>>>(maps[it & 1], ws.inv_s, ws.y[(it + 1) & 1], ws.chan_off, h, w, pitch);
+        IRN_LAUNCH_CHECK("rw_step_tma_kernel");
     }
     return kOk;
-#endif
 }
 
-// Launches the fused walk; *launched = false when the device cannot co-schedule a cluster of the needed size (caller falls
-// back to the per-step kernel).
-template <int PY>
+// Launches the fused walk; *n_clusters = 0 (and nothing launched) when the device cannot co-schedule a cluster of the needed
+// size.
 static int launch_fused(const RwWorkspace& ws, const float* x, const float* edge, float* out, int totc, int h, int w, int n_iter,
-                        cudaStream_t stream, bool* launched, int* n_clusters_out) {
-    *launched = false;
+                        cudaStream_t stream, int* n_clusters) {
+    *n_clusters = 0;
     const int need = (h + kFR - 1) / kFR;
     int cs = 1;
     while (cs < need) cs *= 2;
     static DeviceOnce once;
     const int ds = once.slot();
     if (once.need(ds)) {
-        IRN_CUDA(cudaFuncSetAttribute(rw_fused_kernel<PY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFusedSmem));
-        IRN_CUDA(cudaFuncSetAttribute(rw_fused_kernel<PY>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+        IRN_CUDA(cudaFuncSetAttribute(rw_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFusedSmem));
+        IRN_CUDA(cudaFuncSetAttribute(rw_fused_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
         once.done[ds] = true;
     }
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)cs);
-    cfg.blockDim = dim3(fused_threads(PY));
+    cfg.blockDim = dim3(kFThreads);
     cfg.dynamicSmemBytes = kFusedSmem;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
@@ -905,20 +763,53 @@ static int launch_fused(const RwWorkspace& ws, const float* x, const float* edge
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     int max_clusters = 0;
-    if (cudaOccupancyMaxActiveClusters(&max_clusters, rw_fused_kernel<PY>, &cfg) != cudaSuccess || max_clusters <= 0) {
-        cudaGetLastError();   // not an error of this call: the step kernel takes over
+    if (cudaOccupancyMaxActiveClusters(&max_clusters, rw_fused_kernel, &cfg) != cudaSuccess || max_clusters <= 0) {
+        cudaGetLastError();   // not an error of this call: the caller decides what runs instead
         return kOk;
     }
-    const int n_clusters = totc < max_clusters ? totc : max_clusters;
-    cfg.gridDim = dim3((unsigned)(n_clusters * cs));
+    const int n = totc < max_clusters ? totc : max_clusters;
+    cfg.gridDim = dim3((unsigned)(n * cs));
     const float* Wp = ws.W;
     const double* isp = ws.inv_s;
     const int* cop = ws.chan_off;
     int pitch = ws.pitch;
-    IRN_CUDA(cudaLaunchKernelEx(&cfg, rw_fused_kernel<PY>, Wp, isp, x, edge, out, cop, totc, h, w, pitch, n_iter));
+    IRN_CUDA(cudaLaunchKernelEx(&cfg, rw_fused_kernel, Wp, isp, x, edge, out, cop, totc, h, w, pitch, n_iter));
     IRN_LAUNCH_CHECK("rw_fused_kernel");
-    *launched = true;
-    *n_clusters_out = n_clusters;
+    *n_clusters = n;
+    return kOk;
+}
+
+enum class WalkPath { kFused, kTmaSteps, kGeneric };
+
+// Which kernel walks the batch, decided on the host before any CUDA call, so that a variant that cannot run as asked is
+// refused before anything is launched.
+static int choose_path(int variant, int radius, int h, int w, int n_img, const int32_t* chan_offsets, WalkPath* path) {
+    if (variant == 1 || (variant == 0 && radius != 5)) {
+        *path = WalkPath::kGeneric;
+        return kOk;
+    }
+    if (radius != 5) return fail(kUnsupported, "irn_random_walk_variant: variant %d needs radius 5, got %d", variant, radius);
+    const bool fits = h <= kFR * 16 && w <= kFW;
+    if (variant == 4 && !fits) return fail(kUnsupported, "irn_random_walk: fused walk needs h <= %d, w <= %d", kFR * 16, kFW);
+    if (variant != 0 || !fits) {
+        *path = variant == 4 ? WalkPath::kFused : WalkPath::kTmaSteps;
+        return kOk;
+    }
+    // Both kernels give bit-identical results; pick the faster one from a cost model fitted to H100 measurements
+    // (tools/rw_micro.py, variants 2 and 4, 128x128 grids, 1-4 classes per image): the fused kernel walks one (image, class)
+    // per cluster at ~3.0 us per step on the 7 clusters of 16 CTAs that fit; the per-step kernel shares the weight reads
+    // between up to 4 classes of an image (~1.13 + 0.22 C us per image-chunk per step, ~10 us per step at least).
+    // Single-class images favour the fused kernel, large batches of many-class images (instance path: classes x
+    // instances) the per-step one.
+    double step_us = 0.0;
+    for (int i = 0; i < n_img; ++i) {
+        int c = chan_offsets[i + 1] - chan_offsets[i];
+        for (; c > 0; c -= 4) step_us += 1.13 + 0.22 * (c < 4 ? c : 4);
+    }
+    step_us *= (double)h * w / (128.0 * 128.0);
+    if (step_us < 10.0) step_us = 10.0;
+    const double fused_us = 3.0 * ((chan_offsets[n_img] + 6) / 7);
+    *path = fused_us <= step_us ? WalkPath::kFused : WalkPath::kTmaSteps;
     return kOk;
 }
 
@@ -929,10 +820,24 @@ static thread_local cudaEvent_t g_rw_ev[2] = {nullptr, nullptr};
 static thread_local int g_rw_timed_iters = 0;
 static thread_local int g_rw_last_fused = 0;   // clusters of the last fused launch, 0 = ran step by step
 
+// Records timing event `which` when timing is on: 0 before the walk's step launches, 1 after its `iters` steps.
+static int record_timing(int which, cudaStream_t stream, int iters = 0) {
+    if (!g_rw_timing) return kOk;
+    if (!g_rw_ev[0]) {
+        IRN_CUDA(cudaEventCreate(&g_rw_ev[0]));
+        IRN_CUDA(cudaEventCreate(&g_rw_ev[1]));
+    }
+    IRN_CUDA(cudaEventRecord(g_rw_ev[which], stream));
+    if (which == 1) g_rw_timed_iters = iters;
+    return kOk;
+}
+
 static int walk_impl(const float* x, const float* edge, float* out, int n_img, const int32_t* chan_offsets, int h, int w,
                      int radius, double beta, int n_iter, void* workspace, size_t workspace_bytes, int variant,
                      cudaStream_t stream) {
     launch_counter() = 0;
+    if (variant != 0 && variant != 1 && variant != 2 && variant != 4)
+        return fail(kBadArg, "irn_random_walk_variant: unknown variant %d (0, 1, 2 or 4)", variant);
     if (!x || !edge || !out || !chan_offsets || !workspace) return fail(kBadArg, "irn_random_walk: null pointer");
     if (n_img <= 0 || h <= 0 || w <= 0 || n_iter < 0)
         return fail(kBadArg, "irn_random_walk: bad size (n_img=%d h=%d w=%d n_iter=%d)", n_img, h, w, n_iter);
@@ -945,9 +850,12 @@ static int walk_impl(const float* x, const float* edge, float* out, int n_img, c
     }
     const int totc = chan_offsets[n_img];
     if (totc == 0) return kOk;
+    WalkPath path;
+    int rc = choose_path(variant, radius, h, w, n_img, chan_offsets, &path);
+    if (rc) return rc;
     if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "irn_random_walk: workspace must be 256-byte aligned");
     int n_dst = 0;
-    int rc = upload_tables(radius, stream, &n_dst);
+    rc = upload_tables(radius, stream, &n_dst);
     if (rc) return rc;
     RwWorkspace ws = carve(workspace, n_img, h, w, totc, n_dst);
     if (ws.bytes > workspace_bytes) return fail(kWorkspace, "irn_random_walk: workspace %zu < required %zu bytes", workspace_bytes, ws.bytes);
@@ -958,95 +866,48 @@ static int walk_impl(const float* x, const float* edge, float* out, int n_img, c
     IRN_CUDA(cudaMemcpyAsync(ws.chan_off, chan_offsets, (size_t)(n_img + 1) * sizeof(int), cudaMemcpyHostToDevice, stream));
     const double rb = nearbyint(beta);
     const int ibeta = (rb == beta && beta >= 1 && beta <= 64) ? (int)rb : 0;
-    {
-        const int R = radius - 1;
-        dim3 grid(((w + kAffTX - 1) / kAffTX) * ((h + kAffTY - 1) / kAffTY), n_img), block(kAffTX, kAffTY);
-        const size_t smem = (size_t)(kAffTY + R) * (kAffTX + 2 * R) * sizeof(float);
-        rw_affinity_kernel<0><<<grid, block, smem, stream>>>(edge, ws.W, h, w, pitch, beta, ibeta);
-        IRN_LAUNCH_CHECK("rw_affinity_kernel<0>");
-    }
+    rc = launch_affinity<0>(edge, ws.W, n_img, h, w, pitch, radius, beta, ibeta, stream);
+    if (rc) return rc;
     dim3 pgrid((unsigned)((hw + 255) / 256), n_img);
     rw_rowsum_kernel<<<pgrid, 256, 0, stream>>>(ws.W, ws.inv_s, h, w, pitch);
     IRN_LAUNCH_CHECK("rw_rowsum_kernel");
-    // variant 0: fused cluster kernel when the grid fits (h, w <= 128), else the per-step TMA kernel; 2 forces the per-step
-    // kernel, 4 the fused one
-    bool fused = false;
-    int n_fused_clusters = 0;
-    bool want_fused = radius == 5 && (variant == 0 || variant == 4 || variant == 5) && h <= kFR * 16 && w <= kFW;
-    if (want_fused && variant == 0) {
-        // Both kernels give bit-identical results; pick the faster one from a cost model fitted to H100 measurements
-        // (tools/rw_micro.py, variants 2 and 4, 128x128 grids, 1-4 classes per image): the fused kernel walks one (image, class)
-        // per cluster at ~3.0 us per step on the 7 clusters of 16 CTAs that fit; the per-step kernel shares the weight reads
-        // between up to 4 classes of an image (~1.13 + 0.22 C us per image-chunk per step, ~10 us per step at least).
-        // Single-class images favour the fused kernel, large batches of many-class images (instance path: classes x
-        // instances) the per-step one.
-        double step_us = 0.0;
-        for (int i = 0; i < n_img; ++i) {
-            int c = chan_offsets[i + 1] - chan_offsets[i];
-            for (; c > 0; c -= 4) step_us += 1.13 + 0.22 * (c < 4 ? c : 4);
-        }
-        step_us *= (double)h * w / (128.0 * 128.0);
-        if (step_us < 10.0) step_us = 10.0;
-        const double fused_us = 3.0 * ((totc + 6) / 7);
-        want_fused = fused_us <= step_us;
-    }
-    if (want_fused) {
-        if (g_rw_timing) {
-            if (!g_rw_ev[0]) {
-                IRN_CUDA(cudaEventCreate(&g_rw_ev[0]));
-                IRN_CUDA(cudaEventCreate(&g_rw_ev[1]));
-            }
-            IRN_CUDA(cudaEventRecord(g_rw_ev[0], stream));
-        }
-#ifdef IRN_EXPERIMENTAL
-        rc = variant == 5 ? launch_fused<2>(ws, x, edge, out, totc, h, w, n_iter, stream, &fused, &n_fused_clusters)
-                          : launch_fused<4>(ws, x, edge, out, totc, h, w, n_iter, stream, &fused, &n_fused_clusters);
-#else
-        if (variant == 5) return fail(kUnsupported, "irn_random_walk_variant: variant 5 (two rows per thread) is an experiment, built only with -DIRN_EXPERIMENTAL");
-        rc = launch_fused<4>(ws, x, edge, out, totc, h, w, n_iter, stream, &fused, &n_fused_clusters);
-#endif
+
+    if (path == WalkPath::kFused) {
+        int n_clusters = 0;
+        rc = record_timing(0, stream);
+        if (!rc) rc = launch_fused(ws, x, edge, out, totc, h, w, n_iter, stream, &n_clusters);
         if (rc) return rc;
-        if (fused && g_rw_timing) {
-            IRN_CUDA(cudaEventRecord(g_rw_ev[1], stream));
-            g_rw_timed_iters = n_iter > 0 ? n_iter : 1;
+        if (n_clusters > 0) {
+            g_rw_last_fused = n_clusters;
+            return record_timing(1, stream, n_iter > 0 ? n_iter : 1);
         }
+        if (variant == 4) return fail(kUnsupported, "irn_random_walk: the device cannot co-schedule the fused walk's cluster");
+        path = WalkPath::kTmaSteps;   // variant 0: the per-step kernel takes over
     }
-    if ((variant == 4 || variant == 5) && !fused) return fail(kUnsupported, "irn_random_walk: fused walk needs radius 5, h <= %d, w <= %d and a device that can co-schedule the cluster", kFR * 16, kFW);
-    g_rw_last_fused = fused ? n_fused_clusters : 0;
-    if (fused) return kOk;
+    g_rw_last_fused = 0;
 
     rw_init_kernel<<<pgrid, 256, 0, stream>>>(x, edge, ws.y[0], ws.chan_off, h, w, pitch);
     IRN_LAUNCH_CHECK("rw_init_kernel");
-
-    if (g_rw_timing) {
-        if (!g_rw_ev[0]) {
-            IRN_CUDA(cudaEventCreate(&g_rw_ev[0]));
-            IRN_CUDA(cudaEventCreate(&g_rw_ev[1]));
-        }
-        IRN_CUDA(cudaEventRecord(g_rw_ev[0], stream));
-    }
-    if (radius == 5 && variant != 1) {
-        const int ch = max_c >= 4 ? 4 : max_c;
-        if (ch == 1) rc = launch_tma_steps<1>(ws, n_img, totc, h, w, n_iter, variant, stream);
-        else if (ch == 2) rc = launch_tma_steps<2>(ws, n_img, totc, h, w, n_iter, variant, stream);
-        else if (ch == 3) rc = launch_tma_steps<3>(ws, n_img, totc, h, w, n_iter, variant, stream);
-        else rc = launch_tma_steps<4>(ws, n_img, totc, h, w, n_iter, variant, stream);
-        if (rc) return rc;
-    } else {
+    rc = record_timing(0, stream);
+    if (rc) return rc;
+    if (path == WalkPath::kGeneric) {
         for (int it = 0; it < n_iter; ++it) {
             rw_step_generic_kernel<<<pgrid, 256, 0, stream>>>(ws.W, ws.inv_s, ws.y[it & 1], ws.y[(it + 1) & 1], ws.chan_off, h, w, pitch);
             IRN_LAUNCH_CHECK("rw_step_generic_kernel");
         }
+    } else {
+        const int ch = max_c >= 4 ? 4 : max_c;
+        if (ch == 1) rc = launch_tma_steps<1>(ws, n_img, totc, h, w, n_iter, stream);
+        else if (ch == 2) rc = launch_tma_steps<2>(ws, n_img, totc, h, w, n_iter, stream);
+        else if (ch == 3) rc = launch_tma_steps<3>(ws, n_img, totc, h, w, n_iter, stream);
+        else rc = launch_tma_steps<4>(ws, n_img, totc, h, w, n_iter, stream);
+        if (rc) return rc;
     }
-    if (g_rw_timing) {
-        IRN_CUDA(cudaEventRecord(g_rw_ev[1], stream));
-        g_rw_timed_iters = n_iter;
-    }
-    {
-        const size_t n = (size_t)totc * hw;
-        rw_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(ws.y[n_iter & 1], out, totc, h, w, pitch);
-        IRN_LAUNCH_CHECK("rw_finish_kernel");
-    }
+    rc = record_timing(1, stream, n_iter);
+    if (rc) return rc;
+    const size_t n = (size_t)totc * hw;
+    rw_finish_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(ws.y[n_iter & 1], out, totc, h, w, pitch);
+    IRN_LAUNCH_CHECK("rw_finish_kernel");
     return kOk;
 }
 
@@ -1062,12 +923,7 @@ extern "C" int irn_edge_to_affinity(const float* edge, float* aff, int n_img, in
     if (radius < 2 || radius > 10) return fail(kUnsupported, "irn_edge_to_affinity: radius %d outside [2,10]", radius);
     int rc = upload_tables(radius, stream, nullptr);
     if (rc) return rc;
-    const int R = radius - 1;
-    dim3 grid(((w + kAffTX - 1) / kAffTX) * ((h + kAffTY - 1) / kAffTY), n_img), block(kAffTX, kAffTY);
-    const size_t smem = (size_t)(kAffTY + R) * (kAffTX + 2 * R) * sizeof(float);
-    rw_affinity_kernel<1><<<grid, block, smem, stream>>>(edge, aff, h, w, w, 1.0, 1);
-    IRN_LAUNCH_CHECK("rw_affinity_kernel<1>");
-    return kOk;
+    return launch_affinity<1>(edge, aff, n_img, h, w, w, radius, 1.0, 1, stream);
 }
 
 extern "C" int irn_to_affinity_forward(const float* edge, float* aff, int32_t* arg, int n_img, int h, int w, int radius,
@@ -1140,9 +996,9 @@ extern "C" int irn_random_walk(const float* x, const float* edge, float* out, in
     return walk_impl(x, edge, out, n_img, chan_offsets, h, w, radius, beta, n_iter, workspace, workspace_bytes, 0, (cudaStream_t)stream);
 }
 
-// variant: 0 = production (fused cluster kernel when h,w <= 128, else the per-step TMA kernel), 1 = generic bounds-checked
-// kernel (validation), 2 = per-step TMA kernel, 3 = persistent one-CTA-per-SM TMA-ring step kernel (experiment: 67 vs 50
-// us/step at C=2; kept for A/B measurements), 4 = fused cluster kernel or kUnsupported
+// variant: 0 = production (radius 5: the fused cluster kernel or the per-step TMA kernel, by the cost model in choose_path;
+// other radii: the generic kernel), 1 = generic bounds-checked kernel (validation), 2 = per-step TMA kernel (radius 5) or
+// kUnsupported, 4 = fused cluster kernel or kUnsupported; any other value is kBadArg
 extern "C" int irn_random_walk_variant(const float* x, const float* edge, float* out, int n_img, const int32_t* chan_offsets,
                                        int h, int w, int radius, double beta, int n_iter, void* workspace,
                                        size_t workspace_bytes, int variant, irn_stream_t stream) {

@@ -67,6 +67,24 @@ def test_errors_are_reported(built_lib):
         _lib.check(rc, "irn_path_index_fill")
 
 
+def test_walk_variant_refused_before_any_launch(built_lib):
+    """irn_random_walk_variant checks the kernel choice on the host, before any CUDA call: an unknown variant is kBadArg (-1)
+    and variant 2 (per-step TMA kernel, radius 5 only) at another radius is kUnsupported (-4).  The device pointers are
+    dummies that are never dereferenced, so this runs without a GPU."""
+    import ctypes
+    offs = np.array([0, 2], dtype=np.int32)
+    dummy = ctypes.c_void_p(0x100000)
+    call = lambda variant, radius: built_lib.irn_random_walk_variant(dummy, dummy, dummy, 1, offs.ctypes.data, 16, 16, radius,
+                                                                     10.0, 4, dummy, 1 << 20, variant, None)
+    for variant in (3, 5, 7, -1):
+        assert call(variant, 5) == -1
+        assert built_lib.irn_rw_last_launch_count() == 0
+        assert b"variant %d" % variant in built_lib.irn_last_error()
+    assert call(2, 3) == -4
+    assert built_lib.irn_rw_last_launch_count() == 0
+    assert b"variant 2" in built_lib.irn_last_error() and b"radius 5" in built_lib.irn_last_error()
+
+
 def test_device_entry_points_refuse_cpu_tensors(built_lib):
     import torch
     from irn_b200 import indexing, _lib
