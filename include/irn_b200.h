@@ -203,6 +203,20 @@ int irn_edge_displacement_forward(const irn_net* net, const float* x_nchw, int P
                                   int crop_size, float* edge_out, float* dp_out, void* workspace,
                                   size_t workspace_bytes, irn_stream_t stream);
 
+/* EdgeDisplacement.forward for P images of any sizes (H_i, W_i <= crop_size) in one batch, from the decoded images.
+ *   img_u8     device uint8, img_bytes long: image i is uint8 [H_i,W_i,3] (RGB, HWC) at byte img_offsets[i]
+ *   img_offsets HOST int64 [P];  sizes_hw HOST int32 [P][2] = (H_i, W_i)
+ *   lut768     device fp32 [3][256], irn_normalize_lut's table (the loader's normalisation)
+ *   -> edge fp32 [P,1,fc,fc], dp fp32 [P,2,fc,fc], fc = (crop_size-1)/4+1.
+ * Image i's ceil(H_i/4) x ceil(W_i/4) corner holds, bit for bit, what irn_edge_displacement_forward returns for its scale-1.0
+ * (image, flipped image) pair alone (irn_resize_forward); outside it edge = 1 and dp = 0, which makes the edge map the padded
+ * input of the random walk.  workspace device, 256-byte aligned, >= irn_edge_displacement_ragged_workspace_bytes(P, crop_size). */
+size_t irn_edge_displacement_ragged_workspace_bytes(int P, int crop_size);
+int irn_edge_displacement_forward_ragged(const irn_net* net, const uint8_t* img_u8, size_t img_bytes,
+                                         const int64_t* img_offsets, const int32_t* sizes_hw, int P, int crop_size,
+                                         const float* lut768, float* edge_out, float* dp_out, void* workspace,
+                                         size_t workspace_bytes, irn_stream_t stream);
+
 /* ------------------------------------------------------------------------------------
  * C4  multi-scale CAM merge.  Replaces step/make_cam.py:38-52.
  *   cams: HOST array of n_scales DEVICE pointers, each fp32 [20,hs[s],ws[s]] (CAM.forward outputs);

@@ -52,6 +52,9 @@ SIGNATURES = {
     "irn_edge_displacement_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "irn_edge_displacement_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                               c_size_t, c_void_p]),
+    "irn_edge_displacement_ragged_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "irn_edge_displacement_forward_ragged": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                                     c_void_p, c_void_p, c_size_t, c_void_p]),
     "irn_cam_merge": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                               c_void_p]),
     "irn_find_centroids": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),

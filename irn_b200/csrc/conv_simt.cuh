@@ -380,4 +380,74 @@ __global__ void edge_dp_tail_kernel(const float* __restrict__ e, const float* __
     dp[((size_t)p * 2 + 1) * fh * fw + i] = d0[((size_t)y * Wf + x) * 2 + 1];
 }
 
+// ---- ragged EdgeDisplacement batch: images of different sizes on one crop_size canvas.  The sizes and byte offsets of the images
+// travel as a kernel parameter, kRaggedChunk images per launch.
+constexpr int kRaggedChunk = 128;
+
+struct RaggedChunk {
+    long long off[kRaggedChunk];   // byte offset of image j's uint8 [H,W,3] in the packed buffer
+    int h[kRaggedChunk], w[kRaggedChunk];
+};
+
+// The stem input of images i0 .. i0+n-1 of a ragged batch, straight from the packed uint8 RGB images: sample 2i is image i, sample
+// 2i+1 its W-flip within its own width, both normalised through lut [3][256] (the values the scale-1.0 pyramid holds,
+// irn_resize_forward) and zero outside H_i x W_i.  HALO: the zero-haloed NHWC4 layout nchw_to_nhwc4_halo_kernel writes,
+// [B, Hp = Hc+6, Wp = Wc+8, 4]; otherwise the NHWC layout of nchw_to_nhwc_pad_kernel, [B, Hp = Hc, Wp = Wc, 3].
+// grid (ceil(Hp*Wp / 256), 2n)
+template <bool HALO>
+__global__ void ragged_stem_input_kernel(const uint8_t* __restrict__ img, RaggedChunk r, const float* __restrict__ lut,
+                                         float* __restrict__ out, int i0, int Hp, int Wp) {
+    const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+    if (pix >= Hp * Wp) return;
+    const int s = blockIdx.y, j = s >> 1;
+    const int H = r.h[j], W = r.w[j];
+    const int px = pix % Wp, py = pix / Wp;
+    const int x = HALO ? px - 3 : px, y = HALO ? py - 3 : py;
+    float v0 = 0.f, v1 = 0.f, v2 = 0.f;
+    if (x >= 0 && x < W && y >= 0 && y < H) {
+        const int sx = (s & 1) ? W - 1 - x : x;
+        const uint8_t* p = img + r.off[j] + ((size_t)y * W + sx) * 3;
+        v0 = lut[p[0]];
+        v1 = lut[256 + p[1]];
+        v2 = lut[512 + p[2]];
+    }
+    const size_t o = ((size_t)2 * i0 + s) * Hp * Wp + pix;
+    if (HALO) {
+        reinterpret_cast<float4*>(out)[o] = make_float4(v0, v1, v2, 0.f);
+    } else {
+        float* q = out + o * 3;
+        q[0] = v0; q[1] = v1; q[2] = v2;
+    }
+}
+
+// edge_dp_tail_kernel for pair p = i0 + blockIdx.y of a ragged batch: image p's extent fh x fw = ceil(H_p/4) x ceil(W_p/4) holds what
+// edge_dp_tail_kernel writes for that image alone (the flip is over fw); the rest of the fc x fc grid is edge 1, dp 0, the values
+// the random walk's padding needs (an edge of 1 makes every path through it an affinity of 0).
+//   e NHWC [2P,Hf,Wf,1], d NHWC [2P,Hf,Wf,2]  ->  edge [P,fc,fc], dp [P,2,fc,fc]
+__global__ void edge_dp_tail_ragged_kernel(const float* __restrict__ e, const float* __restrict__ d, float* __restrict__ edge,
+                                           float* __restrict__ dp, int Hf, int Wf, int fc, RaggedChunk r, int i0) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int j = blockIdx.y, p = i0 + j;
+    if (i >= fc * fc) return;
+    const int fh = (r.h[j] - 1) / 4 + 1, fw = (r.w[j] - 1) / 4 + 1;
+    const int y = i / fc, x = i % fc;
+    const size_t plane = (size_t)fc * fc;
+    float* ep = edge + (size_t)p * plane + i;
+    float* dq = dp + (size_t)p * 2 * plane + i;
+    if (y >= fh || x >= fw) {
+        *ep = 1.f;
+        dq[0] = 0.f;
+        dq[plane] = 0.f;
+        return;
+    }
+    const size_t fplane = (size_t)Hf * Wf;
+    const float* e0 = e + (size_t)(2 * p) * fplane;
+    const float* e1 = e0 + fplane;
+    const float* d0 = d + (size_t)(2 * p) * fplane * 2;
+    const float a = e0[(size_t)y * Wf + x] / 2.f + e1[(size_t)y * Wf + (fw - 1 - x)] / 2.f;
+    *ep = 1.f / (1.f + expf(-a));
+    dq[0] = d0[((size_t)y * Wf + x) * 2];
+    dq[plane] = d0[((size_t)y * Wf + x) * 2 + 1];
+}
+
 }  // namespace irn

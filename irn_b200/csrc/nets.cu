@@ -465,14 +465,10 @@ static size_t stem_input_floats(int mode, int B, int Hin, int Win) {
     return mode >= 1 ? stem_halo_floats(B, Hin, Win) : (size_t)B * Hin * Win * 3;
 }
 
-// The stem (`c`, built by build_stem) in `mode`: x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win is laid out in x_in
-// (stem_input_floats), then conv 7x7/s2 + bias + ReLU -> out NHWC [B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), 64]
-static int run_stem(int mode, const Conv& c, const float* x_nchw, int B, int H, int W, int Hin, int Win, float* x_in, float* out,
-                    cudaStream_t st) {
+// The stem's conv 7x7/s2 + bias + ReLU in `mode` on x_in, already laid out as stem_input_floats says for an Hin x Win input ->
+// out NHWC [B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), 64]
+static int run_stem_conv(int mode, const Conv& c, int B, int Hin, int Win, float* x_in, float* out, cudaStream_t st) {
     if (mode >= 1) {
-        const size_t total = (size_t)B * (Hin + 6) * (Win + 8);
-        nchw_to_nhwc4_halo_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, (float4*)x_in, B, H, W, Hin + 6, Win + 8);
-        IRN_LAUNCH_CHECK("nchw_to_nhwc4_halo_kernel");
         CUtensorMap act;
         int rc = stem_map(&act, x_in, B, Hin, Win);
         if (rc) return rc;
@@ -485,17 +481,69 @@ static int run_stem(int mode, const Conv& c, const float* x_nchw, int B, int H, 
         a.Cin = 32;        // 3xTF32: one filter row of 8 taps x 4 channels per k-block
         return launch_tc(false, c.tf32, act, nullptr, a, st);
     }
-    const size_t total = (size_t)B * Hin * Win * 3;
-    nchw_to_nhwc_pad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, x_in, B, 3, H, W, Hin, Win);
-    IRN_LAUNCH_CHECK("nchw_to_nhwc_pad_kernel");
     return run_conv(0, c, x_in, B, Hin, Win, nullptr, out, true, st, nullptr, nullptr);
 }
 
-// Runs input layout transform + stem + maxpool + layer1..4 on x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win.
+// The stem (`c`, built by build_stem) in `mode`: x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win is laid out in x_in
+// (stem_input_floats), then conv 7x7/s2 + bias + ReLU -> out NHWC [B, conv_out(Hin, 7, 2, 3), conv_out(Win, 7, 2, 3), 64]
+static int run_stem(int mode, const Conv& c, const float* x_nchw, int B, int H, int W, int Hin, int Win, float* x_in, float* out,
+                    cudaStream_t st) {
+    if (mode >= 1) {
+        const size_t total = (size_t)B * (Hin + 6) * (Win + 8);
+        nchw_to_nhwc4_halo_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, (float4*)x_in, B, H, W, Hin + 6, Win + 8);
+        IRN_LAUNCH_CHECK("nchw_to_nhwc4_halo_kernel");
+    } else {
+        const size_t total = (size_t)B * Hin * Win * 3;
+        nchw_to_nhwc_pad_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x_nchw, x_in, B, 3, H, W, Hin, Win);
+        IRN_LAUNCH_CHECK("nchw_to_nhwc_pad_kernel");
+    }
+    return run_stem_conv(mode, c, B, Hin, Win, x_in, out, st);
+}
+
+// A ragged batch of P decoded uint8 RGB images (device, packed; HOST offsets and sizes) for the EdgeDisplacement forward
+struct RaggedBatch {
+    const uint8_t* img;
+    const int64_t* off;     // host [P]: byte offset of image i
+    const int32_t* hw;      // host [P][2]: H_i, W_i
+    const float* lut;       // device [3][256] normalisation table (irn_normalize_lut)
+    int P;
+};
+
+// Copies images i0 .. i0+n-1 of `rg` into a kernel parameter block
+static RaggedChunk ragged_chunk(const RaggedBatch& rg, int i0, int n) {
+    RaggedChunk c;
+    for (int j = 0; j < n; ++j) {
+        c.off[j] = rg.off[i0 + j];
+        c.h[j] = rg.hw[2 * (i0 + j)];
+        c.w[j] = rg.hw[2 * (i0 + j) + 1];
+    }
+    return c;
+}
+
+// The stem on a ragged batch: its images (and their W-flips) laid out straight into x_in on the Hin x Win canvas, then run_stem_conv.
+// x_in holds what run_stem builds for the scale-1.0 pyramid of each image, byte for byte.
+static int run_stem_ragged(int mode, const Conv& c, const RaggedBatch& rg, int Hin, int Win, float* x_in, float* out, cudaStream_t st) {
+    const int Hp = mode >= 1 ? Hin + 6 : Hin, Wp = mode >= 1 ? Win + 8 : Win;
+    for (int i0 = 0; i0 < rg.P; i0 += kRaggedChunk) {
+        const int n = std::min(kRaggedChunk, rg.P - i0);
+        const dim3 grid((unsigned)((Hp * Wp + 255) / 256), 2 * n);
+        if (mode >= 1) {
+            ragged_stem_input_kernel<true><<<grid, 256, 0, st>>>(rg.img, ragged_chunk(rg, i0, n), rg.lut, x_in, i0, Hp, Wp);
+            IRN_LAUNCH_CHECK("ragged_stem_input_kernel<halo>");
+        } else {
+            ragged_stem_input_kernel<false><<<grid, 256, 0, st>>>(rg.img, ragged_chunk(rg, i0, n), rg.lut, x_in, i0, Hp, Wp);
+            IRN_LAUNCH_CHECK("ragged_stem_input_kernel<nhwc>");
+        }
+    }
+    return run_stem_conv(mode, c, 2 * rg.P, Hin, Win, x_in, out, st);
+}
+
+// Runs input layout transform + stem + maxpool + layer1..4 on x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win, or, when `rg` is
+// given, on its images and their flips (B = 2 rg->P) each zero-padded to Hin x Win.
 // feats[0] = after maxpool (x1 of IRNet), feats[1..4] = layer outputs.  When `keep` is set every feats[i] lives in
 // its own arena buffer (IRNet taps them); otherwise buffers rotate.
 static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int W, int Hin, int Win, Arena& ar, bool keep,
-                     const float* feats[5], TrunkShapes& sh, cudaStream_t st) {
+                     const float* feats[5], TrunkShapes& sh, cudaStream_t st, const RaggedBatch* rg = nullptr) {
     sh = trunk_shapes(B, Hin, Win);
     float* x_in = ar.take(stem_input_floats(net->conv_mode, B, Hin, Win));
     float* stem_out = ar.take((size_t)B * sh.H1 * sh.W1 * 64);
@@ -505,8 +553,9 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
     float* dsb = ar.take(sh.max_act);
     float* ping[2] = {ar.take(sh.max_act), ar.take(sh.max_act)};
     if (!ar.ok) return fail(kWorkspace, "network workspace too small");
-    int rc;
-    if ((rc = run_stem(net->conv_mode, net->stem, x_nchw, B, H, W, Hin, Win, x_in, stem_out, st))) return rc;
+    int rc = rg ? run_stem_ragged(net->conv_mode, net->stem, *rg, Hin, Win, x_in, stem_out, st)
+                : run_stem(net->conv_mode, net->stem, x_nchw, B, H, W, Hin, Win, x_in, stem_out, st);
+    if (rc) return rc;
     {
         const size_t total = (size_t)B * sh.H2 * sh.W2 * 16;
         maxpool3s2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(stem_out, pool_out, B, sh.H1, sh.W1, 64, sh.H2, sh.W2);
@@ -813,21 +862,14 @@ static int run_head(const irn_net* net, const Head& hd, const float* x, int B, i
     return kOk;
 }
 
-// EdgeDisplacement.forward: x NCHW fp32 [2,3,H,W] (image, flipped image) -> edge [1,fh,fw], dp [2,fh,fw],
-// fh = ceil(H/4), fw = ceil(W/4).  The input is zero-padded to crop_size x crop_size (net/resnet50_irn.py:226).
-extern "C" int irn_edge_displacement_forward(const irn_net* net, const float* x_nchw, int P, int H, int W, int crop_size, float* edge_out,
-                                             float* dp_out, void* workspace, size_t workspace_bytes, irn_stream_t stream_) {
-    cudaStream_t st = (cudaStream_t)stream_;
-    launch_counter() = 0;
-    if (!net || net->kind != 1 || !x_nchw || !edge_out || !dp_out || !workspace) return fail(kBadArg, "irn_edge_displacement_forward: bad argument");
-    if (P <= 0 || H <= 0 || W <= 0 || H > crop_size || W > crop_size || (crop_size % 16) != 0)
-        return fail(kBadArg, "irn_edge_displacement_forward: need P > 0 and 0 < H,W <= crop_size (multiple of 16); got P=%d H=%d W=%d crop=%d", P, H, W, crop_size);
-    if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "irn_edge_displacement_forward: workspace must be 256-byte aligned");
-    const int B = 2 * P, S = crop_size;
-    Arena ar{(char*)workspace, workspace_bytes};
+// Net.forward of IRNet (net/resnet50_irn.py:110-133) on B = 2P samples on the S x S canvas, from x_nchw [B,3,H,W] or the ragged batch
+// `rg` (run_trunk): edge logits -> *elog NHWC [B,h2,w2,1], displacements -> *dlog NHWC [B,h2,w2,2] (both in the arena), h2 x w2 the
+// stride-4 grid
+static int run_irn(const irn_net* net, const float* x_nchw, const RaggedBatch* rg, int B, int H, int W, int S, Arena& ar, float** elog_,
+                   float** dlog_, int* h2_, int* w2_, cudaStream_t st) {
     const float* f[5];
     TrunkShapes sh;
-    int rc = run_trunk(net, x_nchw, B, H, W, S, S, ar, true, f, sh, st);
+    int rc = run_trunk(net, x_nchw, B, H, W, S, S, ar, true, f, sh, st, rg);
     if (rc) return rc;
     const int h2 = sh.Hl[0], w2 = sh.Wl[0];   // stride 4 (x1, x2)
     const int h3 = sh.Hl[1], w3 = sh.Wl[1];   // stride 8 (x3)
@@ -860,9 +902,86 @@ extern "C" int irn_edge_displacement_forward(const irn_net* net, const float* x_
     if ((rc = run_head(net, net->dp[6], dcat2, B, h2, w2, raw, stats, dp7a, h2, w2, 256, 0, st))) return rc;      // dp7 conv/GN/ReLU
     conv1x1_smalln_kernel<2><<<(unsigned)((g2 * 32 + 255) / 256), 256, 0, st>>>(dp7a, net->dp7_w, nullptr, net->mean_shift, dlog, g2, 256);
     IRN_LAUNCH_CHECK("conv1x1_smalln_kernel<2>");
+    *elog_ = elog;
+    *dlog_ = dlog;
+    *h2_ = h2;
+    *w2_ = w2;
+    return kOk;
+}
 
+// EdgeDisplacement.forward: x NCHW fp32 [2,3,H,W] (image, flipped image) -> edge [1,fh,fw], dp [2,fh,fw],
+// fh = ceil(H/4), fw = ceil(W/4).  The input is zero-padded to crop_size x crop_size (net/resnet50_irn.py:226).
+extern "C" int irn_edge_displacement_forward(const irn_net* net, const float* x_nchw, int P, int H, int W, int crop_size, float* edge_out,
+                                             float* dp_out, void* workspace, size_t workspace_bytes, irn_stream_t stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    launch_counter() = 0;
+    if (!net || net->kind != 1 || !x_nchw || !edge_out || !dp_out || !workspace) return fail(kBadArg, "irn_edge_displacement_forward: bad argument");
+    if (P <= 0 || H <= 0 || W <= 0 || H > crop_size || W > crop_size || (crop_size % 16) != 0)
+        return fail(kBadArg, "irn_edge_displacement_forward: need P > 0 and 0 < H,W <= crop_size (multiple of 16); got P=%d H=%d W=%d crop=%d", P, H, W, crop_size);
+    if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "irn_edge_displacement_forward: workspace must be 256-byte aligned");
+    Arena ar{(char*)workspace, workspace_bytes};
+    float *elog, *dlog;
+    int h2, w2;
+    int rc = run_irn(net, x_nchw, nullptr, 2 * P, H, W, crop_size, ar, &elog, &dlog, &h2, &w2, st);
+    if (rc) return rc;
     const int fh = (H - 1) / 4 + 1, fw = (W - 1) / 4 + 1;
     edge_dp_tail_kernel<<<dim3((fh * fw + 255) / 256, P), 256, 0, st>>>(elog, dlog, edge_out, dp_out, h2, w2, fh, fw);
     IRN_LAUNCH_CHECK("edge_dp_tail_kernel");
+    return kOk;
+}
+
+extern "C" size_t irn_edge_displacement_ragged_workspace_bytes(int P, int crop_size) {
+    return irn_edge_displacement_workspace_bytes(P, crop_size, crop_size, crop_size);
+}
+
+// true when p is device (or managed) memory of the CUDA runtime
+static bool is_device_ptr(const void* p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
+// EdgeDisplacement.forward for P images of any sizes <= crop_size in one batch: every image (and its flip) runs on the zero-padded
+// crop_size canvas, as the reference pads each one (net/resnet50_irn.py:226), so each image's ceil(H/4) x ceil(W/4) corner of the
+// fc x fc output is what irn_edge_displacement_forward returns for it alone; outside it edge = 1, dp = 0.
+extern "C" int irn_edge_displacement_forward_ragged(const irn_net* net, const uint8_t* img_u8, size_t img_bytes, const int64_t* img_offsets,
+                                                    const int32_t* sizes_hw, int P, int crop_size, const float* lut768, float* edge_out,
+                                                    float* dp_out, void* workspace, size_t workspace_bytes, irn_stream_t stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    launch_counter() = 0;
+    const char* fn = "irn_edge_displacement_forward_ragged";
+    if (!net || net->kind != 1 || !img_u8 || !img_offsets || !sizes_hw || !lut768 || !edge_out || !dp_out || !workspace)
+        return fail(kBadArg, "%s: bad argument", fn);
+    if (P <= 0 || crop_size <= 0 || (crop_size % 16) != 0)
+        return fail(kBadArg, "%s: need P > 0 and crop_size a positive multiple of 16; got P=%d crop=%d", fn, P, crop_size);
+    for (int i = 0; i < P; ++i) {
+        const int H = sizes_hw[2 * i], W = sizes_hw[2 * i + 1];
+        if (H <= 0 || W <= 0 || H > crop_size || W > crop_size)
+            return fail(kBadArg, "%s: image %d is %dx%d, need 0 < H,W <= crop_size %d", fn, i, H, W, crop_size);
+        const int64_t off = img_offsets[i];
+        if (off < 0 || (uint64_t)off > img_bytes || img_bytes - (uint64_t)off < (uint64_t)H * W * 3)
+            return fail(kBadArg, "%s: image %d (%dx%dx3 bytes at offset %lld) lies outside the %zu-byte image buffer", fn, i, H, W,
+                        (long long)off, img_bytes);
+    }
+    if (!is_device_ptr(img_u8) || !is_device_ptr(lut768) || !is_device_ptr(edge_out) || !is_device_ptr(dp_out) || !is_device_ptr(workspace))
+        return fail(kBadArg, "%s: images, table, outputs and workspace must be device memory", fn);
+    if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "%s: workspace must be 256-byte aligned", fn);
+    if (workspace_bytes < irn_edge_displacement_ragged_workspace_bytes(P, crop_size)) return fail(kWorkspace, "%s: workspace too small", fn);
+    const RaggedBatch rg{img_u8, img_offsets, sizes_hw, lut768, P};
+    Arena ar{(char*)workspace, workspace_bytes};
+    float *elog, *dlog;
+    int h2, w2;
+    int rc = run_irn(net, nullptr, &rg, 2 * P, crop_size, crop_size, crop_size, ar, &elog, &dlog, &h2, &w2, st);
+    if (rc) return rc;
+    const int fc = (crop_size - 1) / 4 + 1;
+    for (int i0 = 0; i0 < P; i0 += kRaggedChunk) {
+        const int n = std::min(kRaggedChunk, P - i0);
+        edge_dp_tail_ragged_kernel<<<dim3((fc * fc + 255) / 256, n), 256, 0, st>>>(elog, dlog, edge_out, dp_out, h2, w2, fc,
+                                                                                   ragged_chunk(rg, i0, n), i0);
+        IRN_LAUNCH_CHECK("edge_dp_tail_ragged_kernel");
+    }
     return kOk;
 }

@@ -8,12 +8,24 @@ model in eval mode, net/resnet50_irn.py:105-108).
 """
 import ctypes
 
+import numpy as np
 import torch
 
-from . import _lib, _pack
+from . import _lib, _pack, preprocess
 from ._params import IrnParams
 from .cam import _Plan
 from .indexing import _workspace
+
+_luts = {}
+
+
+def _normalize_lut(device):
+    """The loader's normalisation table (irn_normalize_lut) on `device`, uploaded once."""
+    t = _luts.get(device)
+    if t is None:
+        t = torch.from_numpy(preprocess.normalize_lut()).to(device)
+        _luts[device] = t
+    return t
 
 
 class EdgeDisplacement(IrnParams):
@@ -68,6 +80,43 @@ class EdgeDisplacement(IrnParams):
             rc = L.irn_edge_displacement_forward(plan.handle, _lib.ptr(x), P, H, W, int(self.crop_size), _lib.ptr(edge), _lib.ptr(dp),
                                                  _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
         _lib.check(rc, "irn_edge_displacement_forward")
+        return edge, dp
+
+    def forward_ragged(self, images, sizes=None):
+        """P decoded images of any sizes <= crop_size in one forward: `images` is a list of uint8 [H_i,W_i,3] RGB tensors, or one
+        flat uint8 cuda tensor holding them back to back with `sizes` = [(H_i, W_i)].  Returns (edge [P,1,fc,fc], dp [P,2,fc,fc]),
+        fc = (crop_size-1)//4+1: image i's ceil(H_i/4) x ceil(W_i/4) corner equals, bit for bit, forward_batch of its scale-1.0
+        (image, flipped image) pair alone; elsewhere edge is 1.0 and dp 0 (the random walk's padding)."""
+        if self.stride != 4:
+            raise _lib.IrnError("EdgeDisplacement: only stride=4 (the reference default) is built")
+        if sizes is None:
+            sizes = [(int(t.shape[0]), int(t.shape[1])) for t in images]
+            flat = torch.cat([t.reshape(-1) for t in images]) if len(images) > 1 else images[0].reshape(-1)
+        else:
+            flat = images
+        sizes = [(int(h), int(w)) for h, w in sizes]
+        P = len(sizes)
+        if P == 0:
+            raise _lib.IrnError("EdgeDisplacement.forward_ragged: empty batch")
+        if flat.dtype != torch.uint8 or flat.dim() != 1:
+            raise _lib.IrnError("EdgeDisplacement.forward_ragged expects uint8 images, got %s %s" % (flat.dtype, tuple(flat.shape)))
+        dev = torch.device("cuda", torch.cuda.current_device()) if not flat.is_cuda else flat.device
+        flat = flat.to(dev, non_blocking=True).contiguous()
+        hw = np.ascontiguousarray(np.asarray(sizes, dtype=np.int32).reshape(P, 2))
+        offs = np.zeros(P, np.int64)
+        np.cumsum(hw[:-1, 0].astype(np.int64) * hw[:-1, 1] * 3, out=offs[1:])
+        L = _lib.lib()
+        plan = self._get_plan(dev)
+        S = int(self.crop_size)
+        fc = (S - 1) // 4 + 1
+        edge = torch.empty((P, 1, fc, fc), dtype=torch.float32, device=dev)
+        dp = torch.empty((P, 2, fc, fc), dtype=torch.float32, device=dev)
+        ws = _workspace(L.irn_edge_displacement_ragged_workspace_bytes(P, S), dev)
+        with torch.cuda.device(dev):
+            rc = L.irn_edge_displacement_forward_ragged(plan.handle, _lib.ptr(flat), flat.numel(), offs.ctypes.data, hw.ctypes.data, P, S,
+                                                        _lib.ptr(_normalize_lut(dev)), _lib.ptr(edge), _lib.ptr(dp), _lib.ptr(ws),
+                                                        ws.numel(), _lib.stream_ptr())
+        _lib.check(rc, "irn_edge_displacement_forward_ragged")
         return edge, dp
 
     def forward(self, x):

@@ -1,15 +1,16 @@
 """Batched pseudo-label pipeline: the reference's make_cam -> make_sem_seg_labels / make_ins_seg_labels chains
 (step/make_cam.py:28-56, step/make_sem_seg_labels.py:28-51, step/make_ins_seg_labels.py:122-152) for a batch of
-equally-sized images, kept on the device end to end (the reference round-trips every image through a .npy file and
-one-image kernels).
+images, kept on the device end to end (the reference round-trips every image through a .npy file and one-image kernels).
+The CAM stages take images of one size; the IRNet, walk, label and instance stages also come in a form for images of
+different sizes on the padded crop_size canvas (*_ragged_stage, walk_padded_stage), exact to the one-size form.
 
     stage                      reference                                    here
     pyramids (C1)              voc12/dataloader.py:191-201                  PseudoLabelPipeline.pyramids
     multi-scale CAM (C2-C4)    step/make_cam.py:35-52                       .cam_stage
-    EdgeDisplacement (I1/I2)   step/make_sem_seg_labels.py:32               .irn_stage
-    random walk (R1-R6)        misc/indexing.py:141-167                     .walk_stage
-    label map (S1)             step/make_sem_seg_labels.py:43-49            .label_stage
-    instances (P1-P4)          step/make_ins_seg_labels.py:131-150          .instance_stage
+    EdgeDisplacement (I1/I2)   step/make_sem_seg_labels.py:32               .irn_stage, .irn_ragged_stage
+    random walk (R1-R6)        misc/indexing.py:141-167                     .walk_stage, .walk_padded_stage
+    label map (S1)             step/make_sem_seg_labels.py:43-49            .label_stage, .label_ragged_stage
+    instances (P1-P4)          step/make_ins_seg_labels.py:131-150          .instance_stage, .instance_ragged_stage
 
 `irn_b200.step.*` drive these stages from the reference's `run(args)` entry points (files in, files out); `run_u8` /
 `run_instances_u8` chain them in memory.
@@ -111,6 +112,72 @@ class PseudoLabelPipeline:
             dps.append(d)
         return (edges[0], dps[0]) if len(edges) == 1 else (torch.cat(edges, 0), torch.cat(dps, 0))
 
+    def irn_ragged_stage(self, images_u8, sizes):
+        """I1/I2 for images of different sizes: images_u8 one flat cuda uint8 buffer holding uint8 [H_i,W_i,3] back to back, sizes
+        [(H_i, W_i)] -> (edge [N,fc,fc], dp [N,2,fc,fc]) on the crop_size canvas (EdgeDisplacement.forward_ragged)."""
+        irn_sub = self.cam_sub * 4
+        offs = np.concatenate([[0], np.cumsum([3 * h * w for h, w in sizes])])
+        edges, dps = [], []
+        for i in range(0, len(sizes), irn_sub):
+            j = min(i + irn_sub, len(sizes))
+            e, d = self.irn.forward_ragged(images_u8[int(offs[i]):int(offs[j])], sizes[i:j])
+            edges.append(e[:, 0])
+            dps.append(d)
+        return (edges[0], dps[0]) if len(edges) == 1 else (torch.cat(edges, 0), torch.cat(dps, 0))
+
+    def walk_padded_stage(self, seeds, edges, sizes):
+        """walk_stage for images of different sizes on the padded grids of irn_ragged_stage: seeds [C_i,fh_i,fw_i] are zero-padded
+        to the edges' fc x fc; returns the list of walks cropped back to [C_i,fh_i,fw_i].  Exactly the walk on each image's own grid:
+        the padded edge is 1.0, so every path into the pad has affinity 0, and a path between two pixels of the image stays inside it."""
+        fc_h, fc_w = int(edges.shape[-2]), int(edges.shape[-1])
+        padded = [torch.nn.functional.pad(s, (0, fc_w - s.shape[-1], 0, fc_h - s.shape[-2])) for s in seeds]
+        rw, counts = self.walk_stage(padded, edges)
+        out, o = [], 0
+        for (h, w), c in zip(sizes, counts):
+            fh, fw = (h - 1) // 4 + 1, (w - 1) // 4 + 1
+            out.append(rw[o:o + c, :fh, :fw])
+            o += c
+        return out
+
+    def label_ragged_stage(self, rws, keys, sizes, bg_thres=None):
+        """S1 for images of different sizes: rws list of [C_i,fh_i,fw_i] walks -> one flat cuda uint8 buffer holding the label maps
+        [H_i,W_i] back to back."""
+        out = torch.empty(sum(h * w for h, w in sizes), dtype=torch.uint8, device=self.device)
+        o = 0
+        for rw, k, (h, w) in zip(rws, keys, sizes):
+            lab = out[o:o + h * w].view(h, w)
+            if rw.shape[0]:
+                indexing.rw_labels(rw, k, (h, w), self.bg if bg_thres is None else bg_thres, out=lab)
+            else:
+                lab.zero_()
+            o += h * w
+        return out
+
+    def instance_ragged_stage(self, strided, keys, edges, dps, sizes, bg_thres=None):
+        """instance_stage for images of different sizes on the padded grids of irn_ragged_stage: the displacement field is cropped to
+        each image's [2,fh_i,fw_i] before the centroid search, the walk runs padded (walk_padded_stage)."""
+        seeds, n_inst = [], []
+        for i, (h, w) in enumerate(sizes):
+            dp = dps[i, :, :(h - 1) // 4 + 1, :(w - 1) // 4 + 1].contiguous()
+            cen = instance.find_centroids_with_refinement(dp)
+            inst_map, I = instance.cluster_centroids(cen, dp)
+            n_inst.append(I)
+            s = instance.separate_score_by_mask(strided[i], inst_map, I)            # [K, I, h, w]
+            seeds.append(s.reshape(-1, s.shape[-2], s.shape[-1]))
+        rws = self.walk_padded_stage(seeds, edges, sizes)
+        return [self._detections(rw, k, I, size, bg_thres) for rw, k, I, size in zip(rws, keys, n_inst, sizes)]
+
+    def _detections(self, rw, keys, n_inst, size, bg_thres):
+        """P4 of one image (step/make_ins_seg_labels.py:137-150): its walk [K*I,h,w] -> the reference's detection dict, None
+        without detections."""
+        if rw.shape[0] == 0:
+            return None
+        _, index, scores = indexing.rw_labels(rw, None, size, self.bg if bg_thres is None else bg_thres, want_index=True, want_scores=True)
+        try:
+            return instance.detect_instance(scores, index, np.repeat(np.asarray(keys), n_inst), max_fragment_size=size[0] * size[1] * 0.01)
+        except ValueError:
+            return None
+
     def walk_stage(self, seeds, edges):
         """R1-R6 batched: seeds = list over images of cuda [C_i,h,w]; edges [N,h,w].  Returns (rw [sum C_i,h,w], counts).
         The fused cluster kernel takes every (image, channel) of a sub-batch in one launch."""
@@ -153,18 +220,8 @@ class PseudoLabelPipeline:
         rw, counts = self.walk_stage(seeds, edges)
         out, o = [], 0
         for i in range(N):
-            c = counts[i]
-            if c == 0:
-                out.append(None)
-                continue
-            _, index, scores = indexing.rw_labels(rw[o:o + c], None, size, self.bg if bg_thres is None else bg_thres, want_index=True,
-                                                  want_scores=True)
-            o += c
-            try:
-                out.append(instance.detect_instance(scores, index, np.repeat(np.asarray(keys[i]), n_inst[i]),
-                                                    max_fragment_size=size[0] * size[1] * 0.01))
-            except ValueError:
-                out.append(None)
+            out.append(self._detections(rw[o:o + counts[i]], keys[i], n_inst[i], size, bg_thres))
+            o += counts[i]
         return out
 
     # ------------------------------------------------------------------ whole chains

@@ -4,12 +4,15 @@ The reference repeats the same skeleton in step/make_cam.py, step/make_sem_seg_l
 step/make_ins_seg_labels.py: build the model class named on the command line, load its checkpoint, split the
 image list over the visible GPUs with the stride partition, spawn one worker per GPU, loop over a batch-size-1
 DataLoader.  Here that skeleton exists once; each step module supplies its per-image function (the reference's loop
-body, one image at a time) and its per-batch function (the same arithmetic for a batch of equally-sized images through
-irn_b200.pipeline, used whenever the loader hands over decoded uint8 images: --device_pyramid, the default).
+body, one image at a time) and its per-batch function (the same arithmetic for a batch of images through irn_b200.pipeline, used
+whenever the loader hands over decoded uint8 images: --device_pyramid, the default).
 
 Batched mode keeps the reference's observable behaviour: same files, same names, same formats; only the order in which
-files appear changes (images are bucketed by size, a bucket is flushed when it holds --step_batch images or at the end),
-and file writes overlap the GPU work of the next batch on a small thread pool.
+files appear changes, and file writes overlap the GPU work of the next batch on a small thread pool.  make_sem_seg_labels and
+make_ins_seg_labels batch images of any sizes (IRNet pads every image to crop_size anyway, and the walk on the padded grid is the
+walk on the image's own grid): a batch is every --step_batch consecutive images.  make_cam and cam_to_ir_label work at each image's
+own size: their images are bucketed by size, a bucket is flushed when it holds --step_batch images, when the pending buckets
+together hold more than PENDING_BOUND x --step_batch images (the largest goes), or at the end (Batcher).
 """
 import contextlib
 import importlib
@@ -110,8 +113,52 @@ def device_jpeg(args):
 
 
 def step_batch(args):
-    """--step_batch N (default 32): images of equal size processed together; 1 = the reference's one-image loop."""
+    """--step_batch N (default 32): images processed together -- of any sizes in make_sem_seg_labels and make_ins_seg_labels, of equal
+    size in make_cam and cam_to_ir_label; 1 = the reference's one-image loop."""
     return max(1, int(getattr(args, "step_batch", DEFAULT_STEP_BATCH) or 1))
+
+
+# a bucketed step holds at most this many times --step_batch images in its pending buckets
+PENDING_BOUND = 4
+
+
+def size_key(pack):
+    return (pack["size"], "jpeg" if "jpeg" in pack else tuple(pack["img_u8"].shape))
+
+
+class Batcher:
+    """Groups a step's items into batches for `per_batch(ctx, packs)`.
+
+    ragged (the steps whose network runs every image on the padded crop_size canvas, make_sem_seg_labels and
+    make_ins_seg_labels): one pending list, flushed every `bsz` items whatever their sizes.
+    Otherwise (make_cam, cam_to_ir_label, whose work runs at each image's own size): one bucket per size, flushed when it holds
+    `bsz` items; when more than PENDING_BOUND * bsz items wait in all buckets together, the largest bucket is flushed early, so a
+    list with many sizes holds a bounded number of items (each keeps its loader chunk's shared memory alive).  finish() flushes
+    what is left.  Every item goes into exactly one batch."""
+
+    def __init__(self, ctx, per_batch, bsz, ragged):
+        self.ctx, self.per_batch, self.bsz, self.ragged = ctx, per_batch, bsz, ragged
+        self.buckets = {}
+        self.pending = 0
+
+    def add(self, pack):
+        key = None if self.ragged else size_key(pack)
+        b = self.buckets.setdefault(key, [])
+        b.append(pack)
+        self.pending += 1
+        if len(b) >= self.bsz:
+            self._flush(key)
+        elif self.pending > PENDING_BOUND * self.bsz:
+            self._flush(max(self.buckets, key=lambda k: len(self.buckets[k])))
+
+    def _flush(self, key):
+        packs = self.buckets.pop(key)
+        self.pending -= len(packs)
+        self.per_batch(self.ctx, packs)
+
+    def finish(self):
+        for key in list(self.buckets):
+            self._flush(key)
 
 
 def make_dataset(args, list_path, scales, cam_dir=None, cam_field="cam", raw_images=False):
@@ -257,6 +304,7 @@ class StepContext:
                                             beta=float(getattr(args, "beta", 10)), exp_times=int(getattr(args, "exp_times", 8)))
         self.writer = Writer(device)
         self._pinned = {}
+        self._flat = {"bufs": [None, None], "done": [None, None], "i": 0}     # pack_images' staging
         self._jpeg = None
         self._copy_pool = ThreadPoolExecutor(max_workers=4)
         self.phase_seconds = {} if os.environ.get("IRN_STEP_PROFILE") else None     # host time per phase of the batch bodies
@@ -278,10 +326,7 @@ class StepContext:
         """The decoded images of a bucket as one device uint8 [N,H,W,3], staged through pinned host memory (two alternating
         buffers per shape; a buffer is rewritten only after the upload that last read it has completed)."""
         if "jpeg" in packs[0]:       # --device_jpeg: file bytes -> nvJPEG -> uint8 [N,H,W,3] in HBM
-            if self._jpeg is None:
-                from ..jpeg import JpegDecoder
-                self._jpeg = JpegDecoder(self.device)
-            return self._jpeg.decode([p["jpeg"] for p in packs], size=packs[0]["size"])
+            return self._jpeg_decoder().decode([p["jpeg"] for p in packs], size=packs[0]["size"])
         N = len(packs)
         shape = (N,) + tuple(packs[0]["img_u8"].shape[1:])
         if shape not in self._pinned and len(self._pinned) >= 8:      # VOC has hundreds of image sizes: bound the pinned pool
@@ -304,6 +349,52 @@ class StepContext:
         ev.record(torch.cuda.current_stream(self.device))
         slot["done"][k] = ev
         return dev
+
+    def _jpeg_decoder(self):
+        if self._jpeg is None:
+            from ..jpeg import JpegDecoder
+            self._jpeg = JpegDecoder(self.device)
+        return self._jpeg
+
+    def pack_images(self, packs):
+        """The decoded images of a batch of any sizes as ONE flat device uint8 buffer, image i's [H_i,W_i,3] bytes back to back in
+        pack order, and the list of (H_i, W_i).  Host images are staged through two alternating pinned buffers that grow to the
+        largest batch; with --device_jpeg every size group is decoded as one nvJPEG batch."""
+        if "jpeg" in packs[0]:
+            sizes = [tuple(p["size"]) for p in packs]
+            groups = {}
+            for i, s in enumerate(sizes):
+                groups.setdefault(s, []).append(i)
+            parts = [None] * len(packs)
+            for s, idx in groups.items():
+                dec = self._jpeg_decoder().decode([packs[i]["jpeg"] for i in idx], size=s)
+                for k, i in enumerate(idx):
+                    parts[i] = dec[k].reshape(-1)
+            return (torch.cat(parts) if len(parts) > 1 else parts[0]), sizes
+        sizes = [(int(p["img_u8"].shape[1]), int(p["img_u8"].shape[2])) for p in packs]
+        n = sum(3 * h * w for h, w in sizes)
+        slot = self._flat
+        k = slot["i"]
+        slot["i"] ^= 1
+        if slot["done"][k] is not None:
+            slot["done"][k].synchronize()
+        if slot["bufs"][k] is None or slot["bufs"][k].numel() < n:
+            slot["bufs"][k] = torch.empty(n, dtype=torch.uint8).pin_memory()
+        buf = slot["bufs"][k][:n]
+        offs = np.concatenate([[0], np.cumsum([3 * h * w for h, w in sizes])])
+
+        def put(i):
+            buf[int(offs[i]):int(offs[i + 1])].copy_(packs[i]["img_u8"].reshape(-1))
+        if len(packs) >= 16:
+            list(self._copy_pool.map(put, range(len(packs))))
+        else:
+            for i in range(len(packs)):
+                put(i)
+        dev = buf.to(self.device, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(self.device))
+        slot["done"][k] = ev
+        return dev, sizes
 
 
 def threaded_loader(shard, n_threads, prefetch):
@@ -328,10 +419,10 @@ def threaded_loader(shard, n_threads, prefetch):
             yield collate_one([item])
 
 
-def work_loop(process_id, model, dataset, args, per_image, per_batch=None):
+def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragged=False):
     """One GPU's share: the reference's `_work(process_id, model, dataset, args)` signature and loop order
     (step/make_cam.py:16-59), with the per-image / per-batch body supplied by the step.  model None: a step without a network
-    (cam_to_ir_label), whose items are the decoded images themselves."""
+    (cam_to_ir_label), whose items are the decoded images themselves.  ragged: per_batch takes images of any sizes (Batcher)."""
     shard = dataset[process_id]
     n_gpus = max(torch.cuda.device_count(), 1)
     scales = getattr(getattr(shard, "dataset", shard), "scales", (1.0,))
@@ -355,7 +446,7 @@ def work_loop(process_id, model, dataset, args, per_image, per_batch=None):
         chunked = True
         if getattr(args, "loader_threads", False):     # slower than forked workers (GIL): off
             loader, chunked = threaded_loader(shard, max(2, args.num_workers // n_gpus), prefetch=2 * bsz), False
-        buckets = {}
+        batcher = Batcher(ctx, per_batch, bsz, ragged)
         prof = os.environ.get("IRN_STEP_PROFILE")          # host-side time split of the loop (development aid), printed to stderr
         t_load = t_body = 0.0
         t_start = t_prev = time.perf_counter()
@@ -365,17 +456,12 @@ def work_loop(process_id, model, dataset, args, per_image, per_batch=None):
                 t_now = time.perf_counter()
                 t_load += t_now - t_prev
                 for pack in (split_chunk(msg) if chunked else (msg,)):
-                    key = (pack["size"], "jpeg" if "jpeg" in pack else tuple(pack["img_u8"].shape))
-                    b = buckets.setdefault(key, [])
-                    b.append(pack)
-                    if len(b) >= bsz:
-                        per_batch(ctx, buckets.pop(key))
+                    batcher.add(pack)
                     progress(process_id, n_gpus, it, len(shard))
                     it += 1
                 t_prev = time.perf_counter()
                 t_body += t_prev - t_now
-            for packs in buckets.values():
-                per_batch(ctx, packs)
+            batcher.finish()
             t_loop = time.perf_counter()
             torch.cuda.synchronize()
             t_sync = time.perf_counter()
@@ -429,17 +515,18 @@ def load_cam_dicts(ctx, packs, names, cam_out_dir, field="cam"):
 
 
 def to_device_list(ctx, tensors):
-    """A list of small host tensors [K_i,h,w] -> list of device views of ONE uploaded buffer (one H2D copy per batch instead of one
+    """A list of small host tensors [K_i,h_i,w_i] -> list of device views of ONE uploaded buffer (one H2D copy per batch instead of one
     per image)."""
-    counts = [int(t.shape[0]) for t in tensors]
+    tensors = [torch.as_tensor(t) for t in tensors]
+    counts = [int(t.numel()) for t in tensors]
     # through PINNED memory (torch's caching host allocator keeps the block alive until the copy has run): a copy from pageable memory
     # is staged in stream order, i.e. the host would sit here until the GPU has finished everything issued before it (the IRNet
-    # forward of the same bucket)
-    staged = torch.empty((sum(counts),) + tuple(tensors[0].shape[1:]), dtype=torch.float32, pin_memory=True)
-    torch.cat([torch.as_tensor(t).float() for t in tensors], 0, out=staged)
+    # forward of the same batch)
+    staged = torch.empty(sum(counts), dtype=torch.float32, pin_memory=True)
+    torch.cat([t.float().reshape(-1) for t in tensors], 0, out=staged)
     dev = staged.to(ctx.device, non_blocking=True)
     out, o = [], 0
-    for c in counts:
-        out.append(dev[o:o + c])
+    for t, c in zip(tensors, counts):
+        out.append(dev[o:o + c].view(t.shape))
         o += c
     return out

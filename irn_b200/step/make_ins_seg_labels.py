@@ -24,16 +24,16 @@ def ins_seg_one_image(model, pack, args):
 
 
 def ins_seg_batch(ctx, packs):
-    """step/make_ins_seg_labels.py:122-152 for a bucket of equally-sized images: one IRNet forward, one batched walk over
-    every (class, instance) channel of the bucket (irn_b200.pipeline.instance_stage)."""
+    """step/make_ins_seg_labels.py:122-152 for a batch of images of any sizes: one IRNet forward on the padded crop_size canvas, one
+    batched walk over every (class, instance) channel of the batch on the padded feature grids
+    (irn_b200.pipeline.instance_ragged_stage)."""
     args = ctx.args
     names = [p["name"][0] for p in packs]
     keys, cams = _common.load_cam_dicts(ctx, packs, names, args.cam_out_dir)
-    x = ctx.stack_images(packs)
-    x1 = ctx.pipe.pyramids(x, (1.0,))[0]
-    edges, dps = ctx.pipe.irn_stage(x1)
+    x, sizes = ctx.pack_images(packs)
+    edges, dps = ctx.pipe.irn_ragged_stage(x, sizes)
     strided = _common.to_device_list(ctx, cams)
-    dets = ctx.pipe.instance_stage(strided, keys, edges, dps, packs[0]["size"], float(args.ins_seg_bg_thres))
+    dets = ctx.pipe.instance_ragged_stage(strided, keys, edges, dps, sizes, float(args.ins_seg_bg_thres))
     for name, det in zip(names, dets):
         if det is None:     # the reference's np.stack([]) raises for an image without any detection
             raise ValueError("need at least one array to stack (no instance detected in %s)" % name)
@@ -41,7 +41,7 @@ def ins_seg_batch(ctx, packs):
 
 
 def _work(process_id, model, dataset, args):
-    _common.work_loop(process_id, model, dataset, args, ins_seg_one_image, ins_seg_batch)
+    _common.work_loop(process_id, model, dataset, args, ins_seg_one_image, ins_seg_batch, ragged=True)
 
 
 def run(args):

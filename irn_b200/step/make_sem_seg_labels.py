@@ -19,38 +19,41 @@ def sem_seg_one_image(model, pack, args):
     Image.fromarray(labels.cpu().numpy()).save(os.path.join(args.sem_seg_out_dir, name + ".png"))
 
 
-def _save(ctx, names, labels, out_dir):
+def _save(ctx, names, labels, sizes, out_dir):
     (lab,) = ctx.writer.to_host([labels])
     lab = lab.numpy()
-    for i, name in enumerate(names):
+    o = 0
+    for name, (h, w) in zip(names, sizes):
         # compress_level 1: same pixels in the file, a quarter of zlib's time on busy label maps (the default 6 made PNG encoding
         # the pacer of the whole step: 21 ms per 512x512 map against ~1 ms of GPU time)
-        ctx.writer.submit_file(lambda a, p: Image.fromarray(a).save(p, compress_level=1), lab[i], os.path.join(out_dir, name + ".png"))
+        ctx.writer.submit_file(lambda a, p: Image.fromarray(a).save(p, compress_level=1), lab[o:o + h * w].reshape(h, w),
+                               os.path.join(out_dir, name + ".png"))
+        o += h * w
 
 
 def sem_seg_batch(ctx, packs):
-    """step/make_sem_seg_labels.py:28-51 for a bucket of equally-sized images: one IRNet forward, one batched walk."""
+    """step/make_sem_seg_labels.py:28-51 for a batch of images of any sizes: one IRNet forward on the padded crop_size canvas, one
+    batched walk on the padded feature grids, each image's walk cropped back to its own grid for the label map."""
     args = ctx.args
     names = [voc_data.decode_int_filename(p["name"][0]) for p in packs]
     with ctx.phase("cam dicts"):
         keys, cams = _common.load_cam_dicts(ctx, packs, names, args.cam_out_dir)
     with ctx.phase("stack + upload images"):
-        x = ctx.stack_images(packs)
+        x, sizes = ctx.pack_images(packs)
     with ctx.phase("irn forward (issue)"):
-        x1 = ctx.pipe.pyramids(x, (1.0,))[0]
-        edges, _ = ctx.pipe.irn_stage(x1)
+        edges, _ = ctx.pipe.irn_ragged_stage(x, sizes)
     with ctx.phase("upload cams"):
         seeds = _common.to_device_list(ctx, cams)
     with ctx.phase("walk (issue)"):
-        rw, counts = ctx.pipe.walk_stage(seeds, edges)
+        rws = ctx.pipe.walk_padded_stage(seeds, edges, sizes)
     with ctx.phase("labels (issue)"):
-        labels = ctx.pipe.label_stage(rw, counts, keys, packs[0]["size"], float(args.sem_seg_bg_thres))
+        labels = ctx.pipe.label_ragged_stage(rws, keys, sizes, float(args.sem_seg_bg_thres))
     with ctx.phase("hand to writer"):
-        ctx.writer.submit(_save, ctx, names, labels, args.sem_seg_out_dir)
+        ctx.writer.submit(_save, ctx, names, labels, sizes, args.sem_seg_out_dir)
 
 
 def _work(process_id, model, dataset, args):
-    _common.work_loop(process_id, model, dataset, args, sem_seg_one_image, sem_seg_batch)
+    _common.work_loop(process_id, model, dataset, args, sem_seg_one_image, sem_seg_batch, ragged=True)
 
 
 def run(args):

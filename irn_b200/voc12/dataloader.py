@@ -122,11 +122,13 @@ def attach_cam(item, cam_dir, field="cam"):
 
 class SyntheticMSF(Dataset):
     """Same item format as VOC12ClassificationDatasetMSF over seeded synthetic images (irn_b200.synth):
-    ids are taken from an image-name list when given, else 2007_000000 + index."""
+    ids are taken from an image-name list when given, else 2007_000000 + index.  `sizes`: a list of (H, W), item i of size
+    sizes[i % len(sizes)] (a list of mixed sizes like VOC's); by default every item is `size`."""
 
     def __init__(self, n_items, size=(512, 512), scales=(1.0,), name_list=None, img_normal=TorchvisionNormalize(), decode_only=False,
-                 cam_dir=None, cam_field="cam"):
+                 cam_dir=None, cam_field="cam", sizes=None):
         self.cam_dir, self.cam_field = cam_dir, cam_field
+        self.sizes = None if sizes is None else [tuple(int(v) for v in s) for s in sizes]
         self.decode_only = decode_only       # (no module stored on the instance: shards are pickled for spawn / DataLoader workers)
         self.n, self.size, self.scales, self.img_normal = n_items, size, scales, img_normal
         self.names = None if name_list is None else load_img_name_list(name_list)[:n_items]
@@ -137,8 +139,9 @@ class SyntheticMSF(Dataset):
     def __getitem__(self, idx):
         name = decode_int_filename(self.names[idx]) if self.names is not None else "2007_%06d" % idx
         from .. import synth
-        img = synth.image(idx, *self.size)
-        out = {"name": name, "size": tuple(self.size), "label": torch.from_numpy(synth.label(idx))}
+        size = tuple(self.size) if self.sizes is None else self.sizes[idx % len(self.sizes)]
+        img = synth.image(idx, *size)
+        out = {"name": name, "size": size, "label": torch.from_numpy(synth.label(idx))}
         if self.decode_only:
             out["img_u8"] = np.array(img)
         else:
