@@ -194,6 +194,15 @@ size_t irn_cam_workspace_bytes(int B, int H, int W);
 int irn_cam_forward(const irn_net* net, const float* x_nchw, int B, int H, int W, float* cam_out,
                     void* workspace, size_t workspace_bytes, irn_stream_t stream);
 
+/* CAM.forward over B/2 pairs of different sizes on one canvas (irn_resize_ragged_forward lays it out).
+ *   x_canvas fp32 [B,3,Hc,Wc] (device), B even: pair p (samples 2p, 2p+1) holds an image of hw[p] = (h_p, w_p) pixels at the
+ *   top-left corner and +0.0 elsewhere; hw HOST int32 [B/2][2], 0 < h_p <= Hc, 0 < w_p <= Wc.
+ *   -> cam fp32 [B/2,20,ceil(Hc/16),ceil(Wc/16)]: pair p's ceil(h_p/16) x ceil(w_p/16) corner is, bit for bit, what irn_cam_forward
+ *   returns for that pair alone (the layers that read beyond an image's extent see zeros there, as they see padding alone); 0
+ *   elsewhere.  workspace device, 256-byte aligned, >= irn_cam_workspace_bytes(B, Hc, Wc). */
+int irn_cam_forward_ragged(const irn_net* net, const float* x_canvas, int B, int Hc, int Wc, const int32_t* hw,
+                           float* cam_out, void* workspace, size_t workspace_bytes, irn_stream_t stream);
+
 /* EdgeDisplacement.forward for P (image, flipped image) pairs of equal size.
  *   x_nchw fp32 [2P,3,H,W]; zero-padded to crop_size (net/resnet50_irn.py:226) ->
  *   edge fp32 [P,1,fh,fw] = sigmoid(e[2p]/2 + e[2p+1].flip(-1)/2), dp fp32 [P,2,fh,fw] = dp[2p] - running_mean;
@@ -285,6 +294,17 @@ int irn_resize_plan_destroy(irn_resize_plan* plan);
 size_t irn_resize_workspace_bytes(const irn_resize_plan* plan, int B);
 int irn_resize_forward(const irn_resize_plan* plan, const uint8_t* img, int B, float* out, uint8_t* out_u8,
                        void* workspace, size_t workspace_bytes, irn_stream_t stream);
+/* irn_resize_ragged_forward   P images of different sizes resized in one call onto one canvas:
+ *                         img_u8 device uint8, img_bytes long: image i is uint8 [H_i,W_i,3] at byte img_offsets[i] (HOST int64 [P]);
+ *                         sizes_hw, out_hw HOST int32 [P][2] = (H_i, W_i), (out_h_i, out_w_i) with out_h_i <= Hc, out_w_i <= Wc;
+ *                         lut768 device fp32 [3][256] (irn_normalize_lut).  out: device fp32 [2P,3,Hc,Wc], rows 2i and 2i+1 =
+ *                         image i and its W-flip within out_w_i, each the out_h_i x out_w_i top-left corner holding what
+ *                         irn_resize_forward writes for that image alone, +0.0 elsewhere.  P <= 65535.  workspace device, 256-byte
+ *                         aligned, >= irn_resize_ragged_workspace_bytes (coefficient tables and the 8-bit intermediate images). */
+size_t irn_resize_ragged_workspace_bytes(const int32_t* sizes_hw, const int32_t* out_hw, int P);
+int irn_resize_ragged_forward(const uint8_t* img_u8, size_t img_bytes, const int64_t* img_offsets, const int32_t* sizes_hw,
+                              const int32_t* out_hw, int P, int Hc, int Wc, const float* lut768, float* out,
+                              void* workspace, size_t workspace_bytes, irn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------
  * N1  JPEG decode on the device (nvJPEG, loaded with dlopen at decoder creation) in place of `imageio.imread` in

@@ -49,6 +49,7 @@ SIGNATURES = {
     "irn_shortcut_conv_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "irn_cam_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "irn_cam_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "irn_cam_forward_ragged": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "irn_edge_displacement_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "irn_edge_displacement_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                               c_size_t, c_void_p]),
@@ -78,6 +79,9 @@ SIGNATURES = {
     "irn_resize_plan_destroy": (c_int, [c_void_p]),
     "irn_resize_workspace_bytes": (c_size_t, [c_void_p, c_int]),
     "irn_resize_forward": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "irn_resize_ragged_workspace_bytes": (c_size_t, [c_void_p, c_void_p, c_int]),
+    "irn_resize_ragged_forward": (c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                          c_void_p, c_size_t, c_void_p]),
     "irn_crf_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
     "irn_crf_max_labels": (c_int, []),
     "irn_dense_crf": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_double, c_float, c_float, c_float, c_float,

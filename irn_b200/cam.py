@@ -8,6 +8,7 @@ BN-folded NHWC convolutions, fused ReLU/residual epilogues and the fused CAM hea
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib, _pack
@@ -80,6 +81,29 @@ class CAM(CamParams):
         with torch.cuda.device(x.device):
             rc = L.irn_cam_forward(plan.handle, _lib.ptr(x), B, H, W, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
         _lib.check(rc, "irn_cam_forward")
+        return out
+
+    def forward_ragged(self, canvas, extents):
+        """Pairs of different sizes in one forward: canvas cuda fp32 [2P,3,Hc,Wc] with pair i's image and its flip of extents[i] =
+        (h_i, w_i) pixels at the top-left corner and +0.0 elsewhere (preprocess.resize_normalize_ragged) -> [P,20,ceil(Hc/16),ceil(Wc/16)]:
+        pair i's ceil(h_i/16) x ceil(w_i/16) corner equals, bit for bit, forward_batch of that pair alone; the rest is 0."""
+        _lib.require_cuda(canvas)
+        if canvas.dim() != 4 or canvas.shape[1] != 3 or canvas.shape[0] % 2 or canvas.dtype != torch.float32:
+            raise _lib.IrnError("CAM.forward_ragged expects fp32 [2P,3,Hc,Wc] (image, flipped image) pairs, got %s %s" %
+                                (canvas.dtype, tuple(canvas.shape)))
+        x = canvas.contiguous()
+        B, _, H, W = x.shape
+        hw = np.ascontiguousarray(np.asarray(extents, dtype=np.int32).reshape(-1, 2))
+        if hw.shape[0] != B // 2:
+            raise _lib.IrnError("CAM.forward_ragged: %d extents for %d pairs" % (hw.shape[0], B // 2))
+        L = _lib.lib()
+        plan = self._get_plan(x.device)
+        out = torch.empty((B // 2, 20, (H - 1) // 16 + 1, (W - 1) // 16 + 1), dtype=torch.float32, device=x.device)
+        ws = _workspace(L.irn_cam_workspace_bytes(B, H, W), x.device)
+        with torch.cuda.device(x.device):
+            rc = L.irn_cam_forward_ragged(plan.handle, _lib.ptr(x), B, H, W, hw.ctypes.data, _lib.ptr(out), _lib.ptr(ws), ws.numel(),
+                                          _lib.stream_ptr())
+        _lib.check(rc, "irn_cam_forward_ragged")
         return out
 
     def forward(self, x):

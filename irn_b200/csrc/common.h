@@ -36,6 +36,16 @@ inline int check_cuda(cudaError_t e, const char* what) {
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// true when p is device (or managed) memory of the CUDA runtime
+inline bool is_device_ptr(const void* p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        return false;
+    }
+    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+
 // cudaFuncSetAttribute and the SM count belong to the CURRENT device: launch helpers keep one flag / value per device so that a
 // process driving several GPUs (one host thread each) configures every one of them.
 struct DeviceOnce {

@@ -450,4 +450,72 @@ __global__ void edge_dp_tail_ragged_kernel(const float* __restrict__ e, const fl
     dq[plane] = d0[((size_t)y * Wf + x) * 2 + 1];
 }
 
+// ---- ragged CAM batch: (image, flipped image) pairs of different sizes at the top-left corner of one canvas.  Pair j of a launch
+// covers h[j] x w[j] pixels of the grid the kernel works on; kRaggedChunk pairs per launch.
+struct PairExtents {
+    int h[kRaggedChunk], w[kRaggedChunk];
+};
+
+// Zeroes the pixels of samples 2(i0+j), 2(i0+j)+1 of x NHWC [B,H,W,C] (C % 4 == 0) that lie outside pair j's extent: rows >= h[j],
+// and columns >= w[j] of the rows above.  No reads: the traffic is the padding's.  grid (ceil(max pad pixels * C/4 / 256), 2n)
+__global__ void zero_outside_kernel(float* __restrict__ x, int H, int W, int C, PairExtents e, int i0) {
+    const int s = blockIdx.y, j = s >> 1;
+    const int h = e.h[j], w = e.w[j], C4 = C >> 2;
+    const size_t right = (size_t)h * (W - w) * C4;           // columns w.. of rows 0..h-1
+    const size_t total = right + (size_t)(H - h) * W * C4;   // + rows h..H-1
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    int y, xx, c4;
+    if (i < right) {
+        c4 = (int)(i % C4);
+        const size_t r = i / C4;
+        y = (int)(r / (W - w));
+        xx = w + (int)(r % (W - w));
+    } else {
+        const size_t k = i - right;
+        c4 = (int)(k % C4);
+        const size_t r = k / C4;
+        y = h + (int)(r / W);
+        xx = (int)(r % W);
+    }
+    reinterpret_cast<float4*>(x + ((((size_t)2 * i0 + s) * H + y) * W + xx) * C)[c4] = make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// cam_flip_add_kernel for pair p = i0 + blockIdx.y of a ragged batch: inside its CAM extent he x we the flipped sample is read at
+// (y, we-1-x), i.e. flipped within the pair's own width; outside the extent the output is 0.  grid (ceil(20*h*w / 256), n)
+__global__ void cam_flip_add_ragged_kernel(const float* __restrict__ t, float* __restrict__ out, int h, int w, int C, PairExtents e, int i0) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 20 * h * w) return;
+    const int j = blockIdx.y, p = i0 + j;
+    const int x = i % w, y = (i / w) % h, n = i / (w * h);
+    const int we = e.w[j];
+    float v = 0.f;
+    if (y < e.h[j] && x < we)
+        v = t[(((size_t)(2 * p) * h + y) * w + x) * C + n] + t[(((size_t)(2 * p + 1) * h + y) * w + (we - 1 - x)) * C + n];
+    out[(size_t)p * 20 * h * w + i] = v;
+}
+
+// cam_head_kernel for pair p = i0 + blockIdx.y of a ragged batch, flipped within the pair's CAM width; 0 outside its extent.
+// grid (ceil(h*w*32 / 256), n)
+__global__ void cam_head_ragged_kernel(const float* __restrict__ feat, const float* __restrict__ w, float* __restrict__ out, int h, int wd,
+                                       int Cin, PairExtents e, int i0) {
+    const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (wid >= h * wd) return;
+    const int j = blockIdx.y, p = i0 + j;
+    const int x = wid % wd, y = wid / wd, we = e.w[j];
+    float* o = out + (size_t)p * 20 * h * wd + (size_t)y * wd + x;
+    if (y >= e.h[j] || x >= we) {
+        if (lane < 20) o[(size_t)lane * h * wd] = 0.f;
+        return;
+    }
+    float a0[20], a1[20];
+    smalln_dot<20>(feat + ((((size_t)(2 * p) * h + y) * wd) + x) * Cin, w, Cin, lane, a0);
+    smalln_dot<20>(feat + ((((size_t)(2 * p + 1) * h + y) * wd) + (we - 1 - x)) * Cin, w, Cin, lane, a1);
+    if (lane == 0) {
+#pragma unroll
+        for (int n = 0; n < 20; ++n) o[(size_t)n * h * wd] = fmaxf(a0[n], 0.f) + fmaxf(a1[n], 0.f);
+    }
+}
+
 }  // namespace irn

@@ -538,12 +538,38 @@ static int run_stem_ragged(int mode, const Conv& c, const RaggedBatch& rg, int H
     return run_stem_conv(mode, c, 2 * rg.P, Hin, Win, x_in, out, st);
 }
 
+// Extent of a pair on the grid `levels` stride-2 operators below the input: every one maps an extent n at the origin to ceil(n/2)
+static inline int level_extent(int n, int levels) { return ((n - 1) >> levels) + 1; }
+
+// Zeroes what lies outside each pair's extent in x NHWC [2P,H,W,C], the grid `levels` stride-2 operators below the input
+// (hw: HOST [P][2] input extents)
+static int mask_outside(float* x, int H, int W, int C, const int32_t* hw, int P, int levels, cudaStream_t st) {
+    for (int i0 = 0; i0 < P; i0 += kRaggedChunk) {
+        const int n = std::min(kRaggedChunk, P - i0);
+        PairExtents e;
+        size_t most = 0;
+        for (int j = 0; j < n; ++j) {
+            e.h[j] = level_extent(hw[2 * (i0 + j)], levels);
+            e.w[j] = level_extent(hw[2 * (i0 + j) + 1], levels);
+            most = std::max(most, ((size_t)H * W - (size_t)e.h[j] * e.w[j]) * (C / 4));
+        }
+        if (most == 0) continue;   // every pair of the chunk fills the grid
+        zero_outside_kernel<<<dim3((unsigned)((most + 255) / 256), 2 * n), 256, 0, st>>>(x, H, W, C, e, i0);
+        IRN_LAUNCH_CHECK("zero_outside_kernel");
+    }
+    return kOk;
+}
+
 // Runs input layout transform + stem + maxpool + layer1..4 on x_nchw [B,3,H,W] zero-padded (logically) to Hin x Win, or, when `rg` is
 // given, on its images and their flips (B = 2 rg->P) each zero-padded to Hin x Win.
 // feats[0] = after maxpool (x1 of IRNet), feats[1..4] = layer outputs.  When `keep` is set every feats[i] lives in
 // its own arena buffer (IRNet taps them); otherwise buffers rotate.
+// `ext` (HOST [B/2][2], or null): pair p of x_nchw holds an image of ext[p] pixels at the top-left corner of the canvas and zeros
+// elsewhere.  Then the stem's output and every block's conv1 output, the only tensors a spatial operator reads beyond an image's
+// extent, are zeroed outside it (mask_outside), so each pair's features inside its extent are those of the pair alone.
 static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int W, int Hin, int Win, Arena& ar, bool keep,
-                     const float* feats[5], TrunkShapes& sh, cudaStream_t st, const RaggedBatch* rg = nullptr) {
+                     const float* feats[5], TrunkShapes& sh, cudaStream_t st, const RaggedBatch* rg = nullptr,
+                     const int32_t* ext = nullptr) {
     sh = trunk_shapes(B, Hin, Win);
     float* x_in = ar.take(stem_input_floats(net->conv_mode, B, Hin, Win));
     float* stem_out = ar.take((size_t)B * sh.H1 * sh.W1 * 64);
@@ -556,6 +582,7 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
     int rc = rg ? run_stem_ragged(net->conv_mode, net->stem, *rg, Hin, Win, x_in, stem_out, st)
                 : run_stem(net->conv_mode, net->stem, x_nchw, B, H, W, Hin, Win, x_in, stem_out, st);
     if (rc) return rc;
+    if (ext && (rc = mask_outside(stem_out, sh.H1, sh.W1, 64, ext, B / 2, 1, st))) return rc;
     {
         const size_t total = (size_t)B * sh.H2 * sh.W2 * 16;
         maxpool3s2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(stem_out, pool_out, B, sh.H1, sh.W1, 64, sh.H2, sh.W2);
@@ -563,14 +590,16 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
     }
     feats[0] = pool_out;
     const float* x = pool_out;
-    int h = sh.H2, w = sh.W2, flip = 0;
+    int h = sh.H2, w = sh.W2, flip = 0, levels = 2;   // levels: stride-2 operators between the input and x
     for (int l = 0; l < 4; ++l) {
         const int nb = (int)net->blocks[l].size();
         for (int b = 0; b < nb; ++b) {
             const Block& blk = net->blocks[l][b];
             int ho, wo;
             if ((rc = run_conv(net->conv_mode, blk.c1, x, B, h, w, nullptr, t1, true, st, nullptr, nullptr))) return rc;
+            if (ext && (rc = mask_outside(t1, h, w, blk.c1.cout, ext, B / 2, levels, st))) return rc;   // conv2 reads one pixel beyond
             if ((rc = run_conv(net->conv_mode, blk.c2, t1, B, h, w, nullptr, t2, true, st, &ho, &wo))) return rc;
+            if (blk.c2.stride == 2) ++levels;
             const bool fused = net->conv_mode == 2 && blk.has_c3ds;
             const float* res = x;
             if (blk.has_ds && !fused) {
@@ -792,18 +821,31 @@ extern "C" size_t irn_cam_workspace_bytes(int B, int H, int W) {
     return (trunk_workspace_floats(B, H, W, false) + (size_t)B * sh.Hl[3] * sh.Wl[3] * 64 + 128) * sizeof(float);
 }
 
-// CAM.forward for P = B/2 (image, flipped image) pairs: x NCHW fp32 [B,3,H,W] -> cam [P,20,ceil(H/16),ceil(W/16)]
-extern "C" int irn_cam_forward(const irn_net* net, const float* x_nchw, int B, int H, int W, float* cam_out, void* workspace,
-                               size_t workspace_bytes, irn_stream_t stream_) {
-    cudaStream_t st = (cudaStream_t)stream_;
-    launch_counter() = 0;
-    if (!net || net->kind != 0 || !x_nchw || !cam_out || !workspace) return fail(kBadArg, "irn_cam_forward: bad argument");
-    if (B <= 0 || (B & 1) || H <= 0 || W <= 0) return fail(kBadArg, "irn_cam_forward: B must be a positive even number (image + flipped image), got B=%d H=%d W=%d", B, H, W);
-    if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "irn_cam_forward: workspace must be 256-byte aligned");
-    Arena ar{(char*)workspace, workspace_bytes};
+// The CAM heads of a ragged batch (ext HOST [P][2] input extents): kernel(e, i0, n) launches the head of pairs i0 .. i0+n-1 with
+// their extents on the CAM grid in e
+template <class Launch>
+static int ragged_heads(const int32_t* ext, int P, Launch kernel) {
+    for (int i0 = 0; i0 < P; i0 += kRaggedChunk) {
+        const int n = std::min(kRaggedChunk, P - i0);
+        PairExtents e;
+        for (int j = 0; j < n; ++j) {
+            e.h[j] = level_extent(ext[2 * (i0 + j)], 4);
+            e.w[j] = level_extent(ext[2 * (i0 + j) + 1], 4);
+        }
+        const int rc = kernel(e, i0, n);
+        if (rc) return rc;
+    }
+    return kOk;
+}
+
+// CAM.forward for P = B/2 (image, flipped image) pairs of x NCHW fp32 [B,3,H,W] -> cam [P,20,ceil(H/16),ceil(W/16)].  With `ext`
+// (HOST [P][2]), pair p is an image of ext[p] pixels at the top-left corner of the canvas, zero elsewhere (run_trunk): each pair's
+// head flips within its own CAM width and writes 0 outside its CAM extent.
+static int run_cam(const irn_net* net, const float* x_nchw, int B, int H, int W, const int32_t* ext, float* cam_out, Arena& ar,
+                   cudaStream_t st) {
     const float* feats[5];
     TrunkShapes sh;
-    int rc = run_trunk(net, x_nchw, B, H, W, H, W, ar, false, feats, sh, st);
+    int rc = run_trunk(net, x_nchw, B, H, W, H, W, ar, false, feats, sh, st, nullptr, ext);
     if (rc) return rc;
     const int P = B / 2, h = sh.Hl[3], w = sh.Wl[3];
     if (net->conv_mode >= 1 && net->cls_conv.tf32.ok) {
@@ -812,15 +854,39 @@ extern "C" int irn_cam_forward(const irn_net* net, const float* x_nchw, int B, i
         float* tmp = ar.take((size_t)B * h * w * 64);
         if (!ar.ok) return fail(kWorkspace, "irn_cam_forward: workspace too small");
         if ((rc = run_conv(net->conv_mode, net->cls_conv, feats[4], B, h, w, nullptr, tmp, true, st, nullptr, nullptr))) return rc;
+        if (ext)
+            return ragged_heads(ext, P, [&](const PairExtents& e, int i0, int n) -> int {
+                cam_flip_add_ragged_kernel<<<dim3((unsigned)((20 * h * w + 255) / 256), n), 256, 0, st>>>(tmp, cam_out, h, w, 64, e, i0);
+                IRN_LAUNCH_CHECK("cam_flip_add_ragged_kernel");
+                return kOk;
+            });
         const size_t total = (size_t)P * 20 * h * w;
         cam_flip_add_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(tmp, cam_out, P, h, w, 64);
         IRN_LAUNCH_CHECK("cam_flip_add_kernel");
         return kOk;
     }
+    if (ext)
+        return ragged_heads(ext, P, [&](const PairExtents& e, int i0, int n) -> int {
+            cam_head_ragged_kernel<<<dim3((unsigned)((h * w * 32 + 255) / 256), n), 256, 0, st>>>(feats[4], net->classifier, cam_out, h, w,
+                                                                                              2048, e, i0);
+            IRN_LAUNCH_CHECK("cam_head_ragged_kernel");
+            return kOk;
+        });
     const size_t warps = (size_t)P * h * w;
     cam_head_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(feats[4], net->classifier, cam_out, P, h, w, 2048);
     IRN_LAUNCH_CHECK("cam_head_kernel");
     return kOk;
+}
+
+// CAM.forward for P = B/2 (image, flipped image) pairs: x NCHW fp32 [B,3,H,W] -> cam [P,20,ceil(H/16),ceil(W/16)]
+extern "C" int irn_cam_forward(const irn_net* net, const float* x_nchw, int B, int H, int W, float* cam_out, void* workspace,
+                               size_t workspace_bytes, irn_stream_t stream_) {
+    launch_counter() = 0;
+    if (!net || net->kind != 0 || !x_nchw || !cam_out || !workspace) return fail(kBadArg, "irn_cam_forward: bad argument");
+    if (B <= 0 || (B & 1) || H <= 0 || W <= 0) return fail(kBadArg, "irn_cam_forward: B must be a positive even number (image + flipped image), got B=%d H=%d W=%d", B, H, W);
+    if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "irn_cam_forward: workspace must be 256-byte aligned");
+    Arena ar{(char*)workspace, workspace_bytes};
+    return run_cam(net, x_nchw, B, H, W, nullptr, cam_out, ar, (cudaStream_t)stream_);
 }
 
 static size_t irn_head_floats(int B, const TrunkShapes& s) {
@@ -934,16 +1000,6 @@ extern "C" size_t irn_edge_displacement_ragged_workspace_bytes(int P, int crop_s
     return irn_edge_displacement_workspace_bytes(P, crop_size, crop_size, crop_size);
 }
 
-// true when p is device (or managed) memory of the CUDA runtime
-static bool is_device_ptr(const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-        cudaGetLastError();
-        return false;
-    }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
-
 // EdgeDisplacement.forward for P images of any sizes <= crop_size in one batch: every image (and its flip) runs on the zero-padded
 // crop_size canvas, as the reference pads each one (net/resnet50_irn.py:226), so each image's ceil(H/4) x ceil(W/4) corner of the
 // fc x fc output is what irn_edge_displacement_forward returns for it alone; outside it edge = 1, dp = 0.
@@ -984,4 +1040,26 @@ extern "C" int irn_edge_displacement_forward_ragged(const irn_net* net, const ui
         IRN_LAUNCH_CHECK("edge_dp_tail_ragged_kernel");
     }
     return kOk;
+}
+
+// CAM.forward for P = B/2 pairs of different sizes on one Hc x Wc canvas (irn_resize_ragged_forward lays it out): pair p holds an
+// image of hw[p] pixels at the top-left corner and zeros elsewhere.  Pair p's ceil(h/16) x ceil(w/16) corner of cam_out equals what
+// irn_cam_forward returns for that pair alone; the rest is 0.
+extern "C" int irn_cam_forward_ragged(const irn_net* net, const float* x_canvas, int B, int Hc, int Wc, const int32_t* hw, float* cam_out,
+                                      void* workspace, size_t workspace_bytes, irn_stream_t stream_) {
+    launch_counter() = 0;
+    const char* fn = "irn_cam_forward_ragged";
+    if (!net || net->kind != 0 || !x_canvas || !hw || !cam_out || !workspace) return fail(kBadArg, "%s: bad argument", fn);
+    if (B <= 0 || (B & 1) || Hc <= 0 || Wc <= 0)
+        return fail(kBadArg, "%s: B must be a positive even number (image + flipped image), got B=%d Hc=%d Wc=%d", fn, B, Hc, Wc);
+    if (is_device_ptr(hw)) return fail(kBadArg, "%s: the extents must be host memory", fn);
+    for (int p = 0; p < B / 2; ++p)
+        if (hw[2 * p] <= 0 || hw[2 * p + 1] <= 0 || hw[2 * p] > Hc || hw[2 * p + 1] > Wc)
+            return fail(kBadArg, "%s: pair %d is %dx%d, need 0 < h <= %d and 0 < w <= %d", fn, p, hw[2 * p], hw[2 * p + 1], Hc, Wc);
+    if (!is_device_ptr(x_canvas) || !is_device_ptr(cam_out) || !is_device_ptr(workspace))
+        return fail(kBadArg, "%s: canvas, output and workspace must be device memory", fn);
+    if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "%s: workspace must be 256-byte aligned", fn);
+    if (workspace_bytes < irn_cam_workspace_bytes(B, Hc, Wc)) return fail(kWorkspace, "%s: workspace too small", fn);
+    Arena ar{(char*)workspace, workspace_bytes};
+    return run_cam(net, x_canvas, B, Hc, Wc, hw, cam_out, ar, (cudaStream_t)stream_);
 }

@@ -1,12 +1,13 @@
 """Batched pseudo-label pipeline: the reference's make_cam -> make_sem_seg_labels / make_ins_seg_labels chains
 (step/make_cam.py:28-56, step/make_sem_seg_labels.py:28-51, step/make_ins_seg_labels.py:122-152) for a batch of
 images, kept on the device end to end (the reference round-trips every image through a .npy file and one-image kernels).
-The CAM stages take images of one size; the IRNet, walk, label and instance stages also come in a form for images of
-different sizes on the padded crop_size canvas (*_ragged_stage, walk_padded_stage), exact to the one-size form.
+Every stage also comes in a form for images of different sizes, exact to the one-size form: the CAM stage on per-sub-batch
+canvases with masked padding (cam_ragged_stage), the IRNet, walk, label and instance stages on the padded crop_size canvas
+(*_ragged_stage, walk_padded_stage).
 
     stage                      reference                                    here
     pyramids (C1)              voc12/dataloader.py:191-201                  PseudoLabelPipeline.pyramids
-    multi-scale CAM (C2-C4)    step/make_cam.py:35-52                       .cam_stage
+    multi-scale CAM (C2-C4)    step/make_cam.py:35-52                       .cam_stage, .cam_ragged_stage
     EdgeDisplacement (I1/I2)   step/make_sem_seg_labels.py:32               .irn_stage, .irn_ragged_stage
     random walk (R1-R6)        misc/indexing.py:141-167                     .walk_stage, .walk_padded_stage
     label map (S1)             step/make_sem_seg_labels.py:43-49            .label_stage, .label_ragged_stage
@@ -96,6 +97,32 @@ class PseudoLabelPipeline:
         keys, strided, highres = [], [], []
         for i in range(N):
             k, lo, hi = cam_ops.merge_cams([c[i] for c in cams], size, labels[i], want_highres=want_highres)
+            keys.append(k.numpy())
+            strided.append(lo)
+            highres.append(hi)
+        return keys, strided, (highres if want_highres else None)
+
+    def cam_ragged_stage(self, images_u8, sizes, labels, want_highres=True, scales=None):
+        """C1-C4 for images of different sizes: images_u8 one flat cuda uint8 buffer holding uint8 [H_i,W_i,3] back to back, sizes
+        [(H_i, W_i)], labels [N,20].  Per scale, the sub-batches of cam_stage, each on a canvas as large as its largest image
+        (preprocess.resize_normalize_ragged, CAM.forward_ragged); then merge + normalise per image on its own corner of the CAMs.
+        Returns what cam_stage returns, each image's entries bit for bit those cam_stage gives for it."""
+        scales = self.scales if scales is None else tuple(scales)
+        sizes = [(int(h), int(w)) for h, w in sizes]
+        N = len(sizes)
+        offs = np.concatenate([[0], np.cumsum([3 * h * w for h, w in sizes])])
+        cams = [[] for _ in range(N)]
+        for s in scales:
+            sub = max(1, int(self.cam_sub * (2.0 / s) ** 2))     # as cam_stage
+            for i in range(0, N, sub):
+                j = min(i + sub, N)
+                canvas, ext = preprocess.resize_normalize_ragged(images_u8[int(offs[i]):int(offs[j])], sizes[i:j], s)
+                out = self.cam.forward_ragged(canvas, ext)
+                for k, (h, w) in enumerate(ext):
+                    cams[i + k].append(out[k, :, :(h - 1) // 16 + 1, :(w - 1) // 16 + 1])
+        keys, strided, highres = [], [], []
+        for i in range(N):
+            k, lo, hi = cam_ops.merge_cams(cams[i], sizes[i], labels[i], want_highres=want_highres)
             keys.append(k.numpy())
             strided.append(lo)
             highres.append(hi)

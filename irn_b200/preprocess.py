@@ -104,3 +104,35 @@ def msf_batch(imgs_u8, scales, mean=MEAN, std=STD):
     """voc12/dataloader.py:191-201 for a batch of equal-sized images: list (one entry per scale) of fp32 [2B,3,h_s,w_s]."""
     H, W = int(imgs_u8.shape[-3]), int(imgs_u8.shape[-2])
     return [resize_normalize(imgs_u8, (H, W) if s == 1 else rescaled_size(H, W, s), mean, std) for s in scales]
+
+
+def resize_normalize_ragged(flat_u8, sizes, scale):
+    """One scale of the pyramids of images of different sizes in one call: flat_u8 cuda uint8 holding the images uint8 [H_i,W_i,3]
+    back to back (StepContext.pack_images), sizes [(H_i, W_i)].  Returns (canvas fp32 [2P,3,Hc,Wc], [(h_i, w_i)]): image i resized to
+    (h_i, w_i) = rescaled_size(H_i, W_i, scale) (itself at scale 1.0) at the top-left corner of rows 2i (as is) and 2i+1 (W-flipped
+    within w_i), +0.0 elsewhere; (Hc, Wc) the largest (h_i, w_i).  Each corner equals resize_normalize of that image alone, bit for bit
+    (the loader's MEAN / STD normalisation)."""
+    from .indexing import _workspace
+    from .irn import _normalize_lut
+    _lib.require_cuda(flat_u8)
+    sizes = [(int(h), int(w)) for h, w in sizes]
+    P = len(sizes)
+    if P == 0:
+        raise _lib.IrnError("resize_normalize_ragged: empty batch")
+    if flat_u8.dtype != torch.uint8 or flat_u8.dim() != 1 or not flat_u8.is_contiguous():
+        raise _lib.IrnError("resize_normalize_ragged: expected one flat contiguous uint8 buffer, got %s %s" % (flat_u8.dtype, tuple(flat_u8.shape)))
+    out_hw = [(H, W) if scale == 1 else rescaled_size(H, W, scale) for H, W in sizes]
+    hw = np.ascontiguousarray(np.asarray(sizes, np.int32).reshape(P, 2))
+    ohw = np.ascontiguousarray(np.asarray(out_hw, np.int32).reshape(P, 2))
+    offs = np.zeros(P, np.int64)
+    np.cumsum(hw[:-1, 0].astype(np.int64) * hw[:-1, 1] * 3, out=offs[1:])
+    Hc, Wc = int(ohw[:, 0].max()), int(ohw[:, 1].max())
+    dev = flat_u8.device
+    L = _lib.lib()
+    out = torch.empty((2 * P, 3, Hc, Wc), dtype=torch.float32, device=dev)
+    ws = _workspace(L.irn_resize_ragged_workspace_bytes(hw.ctypes.data, ohw.ctypes.data, P), dev)
+    with torch.cuda.device(dev):
+        rc = L.irn_resize_ragged_forward(_lib.ptr(flat_u8), flat_u8.numel(), offs.ctypes.data, hw.ctypes.data, ohw.ctypes.data, P, Hc, Wc,
+                                         _lib.ptr(_normalize_lut(dev)), _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
+    _lib.check(rc, "irn_resize_ragged_forward")
+    return out, out_hw

@@ -12,7 +12,9 @@ files appear changes, and file writes overlap the GPU work of the next batch on 
 make_ins_seg_labels batch images of any sizes (IRNet pads every image to crop_size anyway, and the walk on the padded grid is the
 walk on the image's own grid): a batch is every --step_batch consecutive images.  make_cam and cam_to_ir_label work at each image's
 own size: their images are bucketed by size, a bucket is flushed when it holds --step_batch images, when the pending buckets
-together hold more than PENDING_BOUND x --step_batch images (the largest goes), or at the end (Batcher).
+together hold more than PENDING_BOUND x --step_batch images (the largest goes), or at the end (Batcher).  make_cam tops up a bucket
+flushed before it is full with smaller images of other sizes, which its CAM forward runs on the bucket's canvas with the padding
+masked, exactly as at their own size.
 """
 import contextlib
 import importlib
@@ -114,7 +116,8 @@ def device_jpeg(args):
 
 def step_batch(args):
     """--step_batch N (default 32): images processed together -- of any sizes in make_sem_seg_labels and make_ins_seg_labels, of equal
-    size in make_cam and cam_to_ir_label; 1 = the reference's one-image loop."""
+    size in cam_to_ir_label, of equal size in make_cam except when a bucket is topped up with smaller images; 1 = the reference's
+    one-image loop."""
     return max(1, int(getattr(args, "step_batch", DEFAULT_STEP_BATCH) or 1))
 
 
@@ -134,10 +137,16 @@ class Batcher:
     Otherwise (make_cam, cam_to_ir_label, whose work runs at each image's own size): one bucket per size, flushed when it holds
     `bsz` items; when more than PENDING_BOUND * bsz items wait in all buckets together, the largest bucket is flushed early, so a
     list with many sizes holds a bounded number of items (each keeps its loader chunk's shared memory alive).  finish() flushes
-    what is left.  Every item goes into exactly one batch."""
+    what is left.  Every item goes into exactly one batch.
 
-    def __init__(self, ctx, per_batch, bsz, ragged):
-        self.ctx, self.per_batch, self.bsz, self.ragged = ctx, per_batch, bsz, ragged
+    riders (make_cam, whose CAM forward also takes images of different sizes on one canvas): a bucket flushed before it is full
+    (by the bound, or by finish(), largest images first) is topped up to `bsz` items with riders, pending items of other sizes
+    that fit inside its H x W and cover at least half its area, the smallest buckets first.  Such a batch runs on the bucket's
+    canvas, where a rider costs at most twice its own pixels; a full bucket, and so every batch of a one-size list, is as without
+    riders."""
+
+    def __init__(self, ctx, per_batch, bsz, ragged, riders=False):
+        self.ctx, self.per_batch, self.bsz, self.ragged, self.riders = ctx, per_batch, bsz, ragged, riders and not ragged
         self.buckets = {}
         self.pending = 0
 
@@ -153,10 +162,32 @@ class Batcher:
 
     def _flush(self, key):
         packs = self.buckets.pop(key)
+        if self.riders and len(packs) < self.bsz:
+            packs += self._take_riders(key[0], self.bsz - len(packs))
         self.pending -= len(packs)
         self.per_batch(self.ctx, packs)
 
+    def _take_riders(self, size, n):
+        """Up to n pending items of sizes that fit inside `size` = (H, W) with at least half its area, the smallest buckets first."""
+        H, W = size
+        fits = [k for k in self.buckets if k[0][0] <= H and k[0][1] <= W and 2 * k[0][0] * k[0][1] >= H * W]
+        out = []
+        for k in sorted(fits, key=lambda k: len(self.buckets[k])):
+            b = self.buckets[k]
+            take = b[:n - len(out)]
+            out += take
+            del b[:len(take)]
+            if not b:
+                del self.buckets[k]
+            if len(out) == n:
+                break
+        return out
+
     def finish(self):
+        if self.riders:     # the largest images first: every other bucket may still ride with them
+            while self.buckets:
+                self._flush(max(self.buckets, key=lambda k: (k[0][0] * k[0][1], len(self.buckets[k]))))
+            return
         for key in list(self.buckets):
             self._flush(key)
 
@@ -419,10 +450,11 @@ def threaded_loader(shard, n_threads, prefetch):
             yield collate_one([item])
 
 
-def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragged=False):
+def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragged=False, riders=False):
     """One GPU's share: the reference's `_work(process_id, model, dataset, args)` signature and loop order
     (step/make_cam.py:16-59), with the per-image / per-batch body supplied by the step.  model None: a step without a network
-    (cam_to_ir_label), whose items are the decoded images themselves.  ragged: per_batch takes images of any sizes (Batcher)."""
+    (cam_to_ir_label), whose items are the decoded images themselves.  ragged: per_batch takes images of any sizes; riders: size
+    buckets topped up with smaller images when flushed early (Batcher)."""
     shard = dataset[process_id]
     n_gpus = max(torch.cuda.device_count(), 1)
     scales = getattr(getattr(shard, "dataset", shard), "scales", (1.0,))
@@ -446,7 +478,7 @@ def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragge
         chunked = True
         if getattr(args, "loader_threads", False):     # slower than forked workers (GIL): off
             loader, chunked = threaded_loader(shard, max(2, args.num_workers // n_gpus), prefetch=2 * bsz), False
-        batcher = Batcher(ctx, per_batch, bsz, ragged)
+        batcher = Batcher(ctx, per_batch, bsz, ragged, riders)
         prof = os.environ.get("IRN_STEP_PROFILE")          # host-side time split of the loop (development aid), printed to stderr
         t_load = t_body = 0.0
         t_start = t_prev = time.perf_counter()

@@ -19,32 +19,41 @@ def cam_one_image(model, pack, args):
 
 
 def _save(ctx, names, keys, strided, highres, out_dir):
-    """Pool thread: one device->host copy per tensor kind for the whole batch, then one np.save per image."""
-    counts = [int(k.size) for k in keys]
-    lo, hi = ctx.writer.to_host([strided, highres])
-    o = 0
-    for name, k, c in zip(names, keys, counts):
+    """Pool thread: one device->host copy per tensor kind for the whole batch (the images' maps flattened back to back: a batch may
+    mix sizes), then one np.save per image."""
+    lo, hi = ctx.writer.to_host([[t.reshape(-1) for t in strided], [t.reshape(-1) for t in highres]])
+    o = oh = 0
+    for name, k, s, h in zip(names, keys, strided, highres):
         # views of the batch's host buffers: pickling copies them, so the buffers live exactly as long as the last write
         ctx.writer.submit_file(np.save, os.path.join(out_dir, name + ".npy"),
-                               {"keys": torch.from_numpy(k.astype(np.int64)), "cam": lo[o:o + c].clone(), "high_res": hi[o:o + c].numpy()})
-        o += c
+                               {"keys": torch.from_numpy(k.astype(np.int64)), "cam": lo[o:o + s.numel()].view(s.shape).clone(),
+                                "high_res": hi[oh:oh + h.numel()].view(h.shape).numpy()})
+        o += s.numel()
+        oh += h.numel()
 
 
 def cam_batch(ctx, packs):
-    """The same body for a bucket of equally-sized decoded images (irn_b200.pipeline stages C1-C4)."""
+    """The same body for a batch of decoded images (irn_b200.pipeline stages C1-C4): a bucket of one size, or a bucket topped up
+    with smaller images (_common.Batcher), which run on the bucket's canvas (cam_ragged_stage)."""
     args = ctx.args
-    with ctx.phase("stack + upload images"):
-        x = ctx.stack_images(packs)
     labels = torch.cat([p["label"] for p in packs], 0)
-    with ctx.phase("pyramids + cam forward + merge (issue)"):
-        xs = ctx.pipe.pyramids(x, ctx.scales)
-        keys, strided, highres = ctx.pipe.cam_stage(xs, labels, packs[0]["size"], want_highres=True, scales=ctx.scales)
+    if len({_common.size_key(p) for p in packs}) > 1:
+        with ctx.phase("pack + upload images"):
+            flat, sizes = ctx.pack_images(packs)
+        with ctx.phase("ragged pyramids + cam forward + merge (issue)"):
+            keys, strided, highres = ctx.pipe.cam_ragged_stage(flat, sizes, labels, want_highres=True, scales=ctx.scales)
+    else:
+        with ctx.phase("stack + upload images"):
+            x = ctx.stack_images(packs)
+        with ctx.phase("pyramids + cam forward + merge (issue)"):
+            xs = ctx.pipe.pyramids(x, ctx.scales)
+            keys, strided, highres = ctx.pipe.cam_stage(xs, labels, packs[0]["size"], want_highres=True, scales=ctx.scales)
     with ctx.phase("hand to writer"):
         ctx.writer.submit(_save, ctx, [p["name"][0] for p in packs], keys, strided, highres, args.cam_out_dir)
 
 
 def _work(process_id, model, dataset, args):
-    _common.work_loop(process_id, model, dataset, args, cam_one_image, cam_batch)
+    _common.work_loop(process_id, model, dataset, args, cam_one_image, cam_batch, riders=True)
 
 
 def run(args):
