@@ -155,6 +155,38 @@ void irn_net_destroy(irn_net* net);
 int irn_net_set_conv_mode(irn_net* net, int mode);
 int irn_net_get_conv_mode(const irn_net* net);
 
+/* Layer taps (test instrumentation): a forward of `net` copies the named intermediate tensor into `dst` (device, at least the
+ * tensor's bytes; NHWC fp32 with the shape irn_net_tap_shape gives) with a cudaMemcpyAsync on the forward's stream, issued
+ * right after the kernel that produced it and before its arena buffer is reused.  dst = NULL clears the tap.  A forward with
+ * no tap set launches exactly what it launches without this interface.  A tap whose buffer is too small fails the forward.
+ *   trunk (both kinds)  IRN_TAP_STEM  stem conv + ReLU (after the ragged mask), before the max pool
+ *                       IRN_TAP_POOL  max pool output
+ *                       IRN_TAP_BLOCK0 + 3 j + {0, 1, 2}: bottleneck j = 0..15 (layer1.0 .. layer4.2): t1 = relu(bn1(conv1)),
+ *                       t2 = relu(bn2(conv2)), the block output
+ *   CAM                 IRN_TAP_CAM_CLS  relu(classifier) [B,h,w,64] (channels 20..63 zero) in the tensor-core modes 1 and 2;
+ *                       never written in mode 0, whose head kernel keeps it in registers
+ *   IRN                 IRN_TAP_HEAD0 + i: head i's raw 1x1 conv output (i = 0..4 fc_edge1..5, 5..11 fc_dp1..7);
+ *                       IRN_TAP_ECAT the 160-channel edge concat, IRN_TAP_DCAT3 dp3|dp4|dp5, IRN_TAP_DCAT2 dp1|dp2|dp6,
+ *                       IRN_TAP_DP7A relu(gn(fc_dp7 conv)), IRN_TAP_ELOG the edge logits [B,h,w,1], IRN_TAP_DLOG dp [B,h,w,2]
+ * irn_net_tap_shape (host only) gives tap `id`'s NHWC shape for a forward of B samples: kind 0 (CAM) on an H x W input, kind 1
+ * (IRN) on the crop_size x crop_size canvas (H, W unused); it fails for an id the kind does not have. */
+enum {
+    IRN_TAP_STEM = 0,
+    IRN_TAP_POOL = 1,
+    IRN_TAP_BLOCK0 = 2,
+    IRN_TAP_CAM_CLS = 50,
+    IRN_TAP_HEAD0 = 50,
+    IRN_TAP_ECAT = 62,
+    IRN_TAP_DCAT3 = 63,
+    IRN_TAP_DCAT2 = 64,
+    IRN_TAP_DP7A = 65,
+    IRN_TAP_ELOG = 66,
+    IRN_TAP_DLOG = 67,
+    IRN_TAP_COUNT = 68
+};
+int irn_net_set_tap(irn_net* net, int id, float* dst, size_t bytes);
+int irn_net_tap_shape(int kind, int id, int B, int H, int W, int crop_size, int shape[4]);
+
 /* One convolution (+ folded FixedBatchNorm, residual add, ReLU) as a plan of its own: the building block of
  * the two networks above (net/resnet50.py:34-54), exposed for unit tests and for wiring other topologies.
  *   weight_oihw HOST fp32 [cout,cin,k,k]; bn4 HOST fp32 [4,cout] = gamma,beta,running_mean,running_var or NULL.

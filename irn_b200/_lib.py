@@ -38,6 +38,8 @@ SIGNATURES = {
     "irn_net_destroy": (None, [c_void_p]),
     "irn_net_set_conv_mode": (c_int, [c_void_p, c_int]),
     "irn_net_get_conv_mode": (c_int, [c_void_p]),
+    "irn_net_set_tap": (c_int, [c_void_p, c_int, c_void_p, c_size_t]),
+    "irn_net_tap_shape": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _p_int]),
     "irn_conv_create": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
     "irn_conv_destroy": (None, [c_void_p]),
     "irn_conv_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),

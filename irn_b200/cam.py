@@ -29,6 +29,22 @@ class _Plan:
         except Exception:
             pass
 
+    def set_tap(self, tap_id, dst):
+        """irn_net_set_tap: the plan's forwards copy tap `tap_id` into `dst` (contiguous fp32 on the plan's device); None clears it."""
+        if dst is not None:
+            _lib.require_cuda(dst)
+            if dst.dtype != torch.float32 or not dst.is_contiguous() or dst.device != self.device:
+                raise _lib.IrnError("a tap buffer is a contiguous fp32 tensor on %s" % self.device)
+        _lib.check(_lib.lib().irn_net_set_tap(self.handle, int(tap_id), _lib.ptr(dst), 0 if dst is None else dst.numel() * 4),
+                   "irn_net_set_tap")
+
+
+def tap_shape(kind, tap_id, B, H=0, W=0, crop_size=0):
+    """NHWC shape of tap `tap_id` (irn_net_tap_shape) for a forward of B samples: kind 0 = CAM on H x W, 1 = IRNet on crop_size."""
+    shape = (ctypes.c_int * 4)()
+    _lib.check(_lib.lib().irn_net_tap_shape(int(kind), int(tap_id), int(B), int(H), int(W), int(crop_size), shape), "irn_net_tap_shape")
+    return tuple(shape)
+
 
 class CAM(CamParams):
     def __init__(self):
@@ -45,6 +61,14 @@ class CAM(CamParams):
 
     # the reference's Net.train() ignores `mode` (net/resnet50_cam.py:39-43); inference only here
     def train(self, mode=True):
+        return self
+
+    def set_tap(self, tap_id, dst, device=None):
+        """Test instrumentation: from now on, forwards copy layer tap `tap_id` (the IRN_TAP_* ids of include/irn_b200.h) into `dst`,
+        a contiguous fp32 cuda tensor of tap_shape(0, tap_id, ...) elements or more; dst None clears the tap.  Taps belong to the
+        current plan: load_state_dict drops them."""
+        dev = dst.device if dst is not None else (device or torch.device("cuda", torch.cuda.current_device()))
+        self._get_plan(dev).set_tap(tap_id, dst)
         return self
 
     def _invalidate(self):

@@ -170,7 +170,8 @@ __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float((__fl
 
 // (a, b) -> packed fp16 pair {low half = hi(a), high half = hi(b)} and the packed pair of the residuals.  hi(x) = x truncated to 11
 // significant bits (round-toward-zero conversion); the same value rebuilt in fp32 by a mask gives the residual x - hi(x), exact in
-// fp32 and rounded once, to 11 bits, by its own conversion: |error| <= 2^-21 |x| for 2^-14 <= |x| <= 65504.
+// fp32 and rounded once, to 11 bits, by its own conversion: |error| <= 2^-21 |x| for 2^-4 <= |x| <= 65504.  Below 2^-4 the residual
+// (< 2^-10 |x| < 2^-14) is an fp16 subnormal: the error is up to 2^-25 absolute, and 2^-24 below 2^-14 where hi(x) is subnormal too.
 __device__ __forceinline__ void f16_split2(float a, float b, uint32_t& hi, uint32_t& lo) {
     asm("cvt.rz.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(b), "f"(a));      // upper half <- first source operand
     const float ha = __uint_as_float(__float_as_uint(a) & 0xFFFFE000u), hb = __uint_as_float(__float_as_uint(b) & 0xFFFFE000u);

@@ -79,6 +79,11 @@ struct irn_net {
     float* edge6_b = nullptr;      // [1]
     float* dp7_w = nullptr;        // [2][256]
     float* mean_shift = nullptr;   // [2]
+    struct Tap {
+        float* dst = nullptr;
+        size_t bytes = 0;
+    };
+    Tap taps[IRN_TAP_COUNT];       // irn_net_set_tap
     irn::DeviceAllocs mem;
 };
 
@@ -307,6 +312,15 @@ static int read_head(DeviceAllocs& mem, Reader& rd, Head& h, int cin, int cout, 
 
 // ------------------------------------------------------------------ launch helpers
 static inline int conv_out(int n, int k, int s, int p) { return (n + 2 * p - k) / s + 1; }
+
+// Copies tap `id`'s tensor, n floats at src, into the caller's buffer when one is set (irn_net_set_tap); nothing otherwise
+static int tap(const irn_net* net, int id, const float* src, size_t n, cudaStream_t st) {
+    const irn_net::Tap& t = net->taps[id];
+    if (!t.dst) return kOk;
+    if (t.bytes < n * sizeof(float)) return fail(kBadArg, "tap %d: buffer of %zu bytes, the tensor has %zu", id, t.bytes, n * sizeof(float));
+    IRN_CUDA(cudaMemcpyAsync(t.dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return kOk;
+}
 
 template <bool F16, int BN>
 static int launch_wg(const TcMaps& maps, const TcArgs& a, cudaStream_t st) {
@@ -583,14 +597,17 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
                 : run_stem(net->conv_mode, net->stem, x_nchw, B, H, W, Hin, Win, x_in, stem_out, st);
     if (rc) return rc;
     if (ext && (rc = mask_outside(stem_out, sh.H1, sh.W1, 64, ext, B / 2, 1, st))) return rc;
+    if ((rc = tap(net, IRN_TAP_STEM, stem_out, (size_t)B * sh.H1 * sh.W1 * 64, st))) return rc;
     {
         const size_t total = (size_t)B * sh.H2 * sh.W2 * 16;
         maxpool3s2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(stem_out, pool_out, B, sh.H1, sh.W1, 64, sh.H2, sh.W2);
         IRN_LAUNCH_CHECK("maxpool3s2_kernel");
     }
+    if ((rc = tap(net, IRN_TAP_POOL, pool_out, (size_t)B * sh.H2 * sh.W2 * 64, st))) return rc;
     feats[0] = pool_out;
     const float* x = pool_out;
     int h = sh.H2, w = sh.W2, flip = 0, levels = 2;   // levels: stride-2 operators between the input and x
+    int tj = IRN_TAP_BLOCK0;                           // the taps of the next block: t1, t2, output
     for (int l = 0; l < 4; ++l) {
         const int nb = (int)net->blocks[l].size();
         for (int b = 0; b < nb; ++b) {
@@ -598,7 +615,9 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
             int ho, wo;
             if ((rc = run_conv(net->conv_mode, blk.c1, x, B, h, w, nullptr, t1, true, st, nullptr, nullptr))) return rc;
             if (ext && (rc = mask_outside(t1, h, w, blk.c1.cout, ext, B / 2, levels, st))) return rc;   // conv2 reads one pixel beyond
+            if ((rc = tap(net, tj, t1, (size_t)B * h * w * blk.c1.cout, st))) return rc;
             if ((rc = run_conv(net->conv_mode, blk.c2, t1, B, h, w, nullptr, t2, true, st, &ho, &wo))) return rc;
+            if ((rc = tap(net, tj + 1, t2, (size_t)B * ho * wo * blk.c2.cout, st))) return rc;
             if (blk.c2.stride == 2) ++levels;
             const bool fused = net->conv_mode == 2 && blk.has_c3ds;
             const float* res = x;
@@ -617,6 +636,8 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
             if (fused) {
                 if ((rc = run_c3ds(blk, t2, x, B, h, w, ho, wo, out, st))) return rc;
             } else if ((rc = run_conv(net->conv_mode, blk.c3, t2, B, ho, wo, res, out, true, st, nullptr, nullptr))) return rc;   // out += residual; relu (net/resnet50.py:51-52)
+            if ((rc = tap(net, tj + 2, out, (size_t)B * ho * wo * blk.c3.cout, st))) return rc;
+            tj += 3;
             x = out;
             h = ho;
             w = wo;
@@ -763,6 +784,49 @@ extern "C" int irn_net_set_conv_mode(irn_net* net, int mode) {
 
 extern "C" int irn_net_get_conv_mode(const irn_net* net) { return net ? net->conv_mode : -1; }
 
+extern "C" int irn_net_set_tap(irn_net* net, int id, float* dst, size_t bytes) {
+    if (!net || id < 0 || id >= IRN_TAP_COUNT || (net->kind == 0 && id > IRN_TAP_CAM_CLS))
+        return fail(kBadArg, "irn_net_set_tap: no tap %d on this network", id);
+    net->taps[id].dst = dst;
+    net->taps[id].bytes = dst ? bytes : 0;
+    return kOk;
+}
+
+extern "C" int irn_net_tap_shape(int kind, int id, int B, int H, int W, int crop_size, int shape[4]) {
+    if (!shape || !(kind == 0 || kind == 1) || B <= 0) return fail(kBadArg, "irn_net_tap_shape: bad argument");
+    if (kind == 1) H = W = crop_size;
+    if (H <= 0 || W <= 0) return fail(kBadArg, "irn_net_tap_shape: bad input size %d x %d", H, W);
+    const TrunkShapes s = trunk_shapes(B, H, W);
+    int h = 0, w = 0, c = 0;
+    if (id == IRN_TAP_STEM || id == IRN_TAP_POOL) {
+        h = id == IRN_TAP_STEM ? s.H1 : s.H2;
+        w = id == IRN_TAP_STEM ? s.W1 : s.W2;
+        c = 64;
+    } else if (id >= IRN_TAP_BLOCK0 && id < IRN_TAP_BLOCK0 + 48) {
+        int j = (id - IRN_TAP_BLOCK0) / 3, l = 0;
+        while (j >= kBlocks[l]) j -= kBlocks[l++];
+        const int which = (id - IRN_TAP_BLOCK0) % 3;
+        const bool in_grid = which == 0 && j == 0;   // conv1 of a stage's first block runs on the previous stage's grid
+        h = in_grid ? (l ? s.Hl[l - 1] : s.H2) : s.Hl[l];
+        w = in_grid ? (l ? s.Wl[l - 1] : s.W2) : s.Wl[l];
+        c = which == 2 ? 4 * kPlanes[l] : kPlanes[l];
+    } else if (kind == 0 && id == IRN_TAP_CAM_CLS) {
+        h = s.Hl[3]; w = s.Wl[3]; c = 64;
+    } else if (kind == 1 && id >= IRN_TAP_HEAD0 && id < IRN_TAP_COUNT) {
+        // grid of each head's conv (edge1..5, dp1..7) and its channels; then ecat, dcat3, dcat2, dp7a, elog, dlog
+        static const int lvl[18] = {0, 1, 2, 3, 3, 0, 1, 2, 3, 3, 2, 1, 1, 2, 1, 1, 1, 1};   // 0 = x1 grid, 1..3 = Hl[0..2]
+        static const int ch[18] = {32, 32, 32, 32, 32, 64, 128, 256, 256, 256, 256, 256, 160, 768, 448, 256, 1, 2};
+        const int i = id - IRN_TAP_HEAD0;
+        h = lvl[i] ? s.Hl[lvl[i] - 1] : s.H2;
+        w = lvl[i] ? s.Wl[lvl[i] - 1] : s.W2;
+        c = ch[i];
+    } else {
+        return fail(kBadArg, "irn_net_tap_shape: no tap %d on a network of kind %d", id, kind);
+    }
+    shape[0] = B; shape[1] = h; shape[2] = w; shape[3] = c;
+    return kOk;
+}
+
 extern "C" void irn_net_destroy(irn_net* net) { delete net; }
 
 extern "C" int irn_cam_net_create(const float* params, size_t n_floats, irn_net** out) {
@@ -854,6 +918,7 @@ static int run_cam(const irn_net* net, const float* x_nchw, int B, int H, int W,
         float* tmp = ar.take((size_t)B * h * w * 64);
         if (!ar.ok) return fail(kWorkspace, "irn_cam_forward: workspace too small");
         if ((rc = run_conv(net->conv_mode, net->cls_conv, feats[4], B, h, w, nullptr, tmp, true, st, nullptr, nullptr))) return rc;
+        if ((rc = tap(net, IRN_TAP_CAM_CLS, tmp, (size_t)B * h * w * 64, st))) return rc;
         if (ext)
             return ragged_heads(ext, P, [&](const PairExtents& e, int i0, int n) -> int {
                 cam_flip_add_ragged_kernel<<<dim3((unsigned)((20 * h * w + 255) / 256), n), 256, 0, st>>>(tmp, cam_out, h, w, 64, e, i0);
@@ -910,10 +975,12 @@ extern "C" size_t irn_edge_displacement_workspace_bytes(int P, int H, int W, int
     return (trunk_workspace_floats(B, crop_size, crop_size, true) + irn_head_floats(B, s) + 64) * sizeof(float);
 }
 
-static int run_head(const irn_net* net, const Head& hd, const float* x, int B, int H, int W, float* raw, float* stats, float* dst, int Hd, int Wd, int Cd,
-                    int coff, cudaStream_t st) {
+// One head (conv1x1 -> GroupNorm -> upsample -> ReLU) into channels [coff, coff + cout) of dst; `id` is the tap of its raw conv output
+static int run_head(const irn_net* net, int id, const Head& hd, const float* x, int B, int H, int W, float* raw, float* stats, float* dst, int Hd,
+                    int Wd, int Cd, int coff, cudaStream_t st) {
     int rc = run_conv(net->conv_mode, hd.conv, x, B, H, W, nullptr, raw, false, st, nullptr, nullptr);
     if (rc) return rc;
+    if ((rc = tap(net, id, raw, (size_t)B * H * W * hd.conv.cout, st))) return rc;
     if (hd.conv.cout > 256 || 256 % hd.conv.cout != 0 || hd.groups > 16) return fail(kUnsupported, "GroupNorm head with %d channels / %d groups", hd.conv.cout, hd.groups);
     IRN_CUDA(cudaMemsetAsync(stats, 0, (size_t)B * hd.groups * 2 * sizeof(double), st));
     {
@@ -954,20 +1021,27 @@ static int run_irn(const irn_net* net, const float* x_nchw, const RaggedBatch* r
     // edge branch (net/resnet50_irn.py:117-122): every map lands on the stride-4 grid, cropped to edge2's size
     const int eh[5] = {h2, h2, h3, h4, h4}, ew[5] = {w2, w2, w3, w4, w4};
     for (int i = 0; i < 5; ++i)
-        if ((rc = run_head(net, net->edge[i], f[i], B, eh[i], ew[i], raw, stats, ecat, h2, w2, 160, 32 * i, st))) return rc;
+        if ((rc = run_head(net, IRN_TAP_HEAD0 + i, net->edge[i], f[i], B, eh[i], ew[i], raw, stats, ecat, h2, w2, 160, 32 * i, st))) return rc;
+    if ((rc = tap(net, IRN_TAP_ECAT, ecat, g2 * 160, st))) return rc;
     conv1x1_smalln_kernel<1><<<(unsigned)((g2 * 32 + 255) / 256), 256, 0, st>>>(ecat, net->edge6_w, net->edge6_b, nullptr, elog, g2, 160);
     IRN_LAUNCH_CHECK("conv1x1_smalln_kernel<1>");
+    if ((rc = tap(net, IRN_TAP_ELOG, elog, g2, st))) return rc;
 
     // displacement branch (net/resnet50_irn.py:124-131)
-    if ((rc = run_head(net, net->dp[0], f[0], B, h2, w2, raw, stats, dcat2, h2, w2, 448, 0, st))) return rc;      // dp1 64
-    if ((rc = run_head(net, net->dp[1], f[1], B, h2, w2, raw, stats, dcat2, h2, w2, 448, 64, st))) return rc;     // dp2 128
-    if ((rc = run_head(net, net->dp[2], f[2], B, h3, w3, raw, stats, dcat3, h3, w3, 768, 0, st))) return rc;      // dp3
-    if ((rc = run_head(net, net->dp[3], f[3], B, h4, w4, raw, stats, dcat3, h3, w3, 768, 256, st))) return rc;    // dp4 up x2, crop to dp3
-    if ((rc = run_head(net, net->dp[4], f[4], B, h4, w4, raw, stats, dcat3, h3, w3, 768, 512, st))) return rc;    // dp5 up x2
-    if ((rc = run_head(net, net->dp[5], dcat3, B, h3, w3, raw, stats, dcat2, h2, w2, 448, 192, st))) return rc;   // dp6 up x2, crop to dp2
-    if ((rc = run_head(net, net->dp[6], dcat2, B, h2, w2, raw, stats, dp7a, h2, w2, 256, 0, st))) return rc;      // dp7 conv/GN/ReLU
+    const int d = IRN_TAP_HEAD0 + 5;
+    if ((rc = run_head(net, d, net->dp[0], f[0], B, h2, w2, raw, stats, dcat2, h2, w2, 448, 0, st))) return rc;           // dp1 64
+    if ((rc = run_head(net, d + 1, net->dp[1], f[1], B, h2, w2, raw, stats, dcat2, h2, w2, 448, 64, st))) return rc;      // dp2 128
+    if ((rc = run_head(net, d + 2, net->dp[2], f[2], B, h3, w3, raw, stats, dcat3, h3, w3, 768, 0, st))) return rc;       // dp3
+    if ((rc = run_head(net, d + 3, net->dp[3], f[3], B, h4, w4, raw, stats, dcat3, h3, w3, 768, 256, st))) return rc;     // dp4 up x2, crop to dp3
+    if ((rc = run_head(net, d + 4, net->dp[4], f[4], B, h4, w4, raw, stats, dcat3, h3, w3, 768, 512, st))) return rc;     // dp5 up x2
+    if ((rc = tap(net, IRN_TAP_DCAT3, dcat3, g3 * 768, st))) return rc;
+    if ((rc = run_head(net, d + 5, net->dp[5], dcat3, B, h3, w3, raw, stats, dcat2, h2, w2, 448, 192, st))) return rc;    // dp6 up x2, crop to dp2
+    if ((rc = tap(net, IRN_TAP_DCAT2, dcat2, g2 * 448, st))) return rc;
+    if ((rc = run_head(net, d + 6, net->dp[6], dcat2, B, h2, w2, raw, stats, dp7a, h2, w2, 256, 0, st))) return rc;       // dp7 conv/GN/ReLU
+    if ((rc = tap(net, IRN_TAP_DP7A, dp7a, g2 * 256, st))) return rc;
     conv1x1_smalln_kernel<2><<<(unsigned)((g2 * 32 + 255) / 256), 256, 0, st>>>(dp7a, net->dp7_w, nullptr, net->mean_shift, dlog, g2, 256);
     IRN_LAUNCH_CHECK("conv1x1_smalln_kernel<2>");
+    if ((rc = tap(net, IRN_TAP_DLOG, dlog, g2 * 2, st))) return rc;
     *elog_ = elog;
     *dlog_ = dlog;
     *h2_ = h2;

@@ -43,6 +43,13 @@ class EdgeDisplacement(IrnParams):
             _lib.check(_lib.lib().irn_net_set_conv_mode(self._plan.handle, self._conv_mode), "irn_net_set_conv_mode")
         return self
 
+    def set_tap(self, tap_id, dst, device=None):
+        """Test instrumentation, as CAM.set_tap: forwards copy tap `tap_id` (shape: cam.tap_shape(1, tap_id, 2P, crop_size=...))
+        into `dst`; None clears it."""
+        dev = dst.device if dst is not None else (device or torch.device("cuda", torch.cuda.current_device()))
+        self._get_plan(dev).set_tap(tap_id, dst)
+        return self
+
     def load_state_dict(self, *a, **k):
         self._plan = None
         return super().load_state_dict(*a, **k)
