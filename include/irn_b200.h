@@ -343,7 +343,7 @@ int irn_resize_ragged_forward(const uint8_t* img_u8, size_t img_bytes, const int
  * VOC12ClassificationDatasetMSF.__getitem__ (voc12/dataloader.py:189): n JPEG streams of one size (host pointers) ->
  * uint8 [n,H,W,3] RGB in HBM, the input layout of irn_resize_forward.  backend 0 = nvJPEG's default GPU-assisted decoder,
  * 1 = the hardware JPEG engine when the device has one (falls back to 0; irn_jpeg_decoder_backend tells).  NOT bit-identical
- * to libjpeg-turbo (+-1..2 levels): a throughput option, parity runs decode on the host.
+ * to libjpeg-turbo (+-1..2 levels): a throughput option; parity runs decode on the host or with irn_jpeg_exact_* below.
  */
 typedef struct irn_jpeg irn_jpeg;
 int irn_jpeg_decoder_create(int backend, irn_jpeg** out);
@@ -352,6 +352,32 @@ void irn_jpeg_decoder_destroy(irn_jpeg* decoder);
 int irn_jpeg_image_size(irn_jpeg* decoder, const uint8_t* data, size_t length, int* H, int* W, int* n_components);
 int irn_jpeg_decode_batch(irn_jpeg* decoder, const uint8_t* const* data, const size_t* lengths, int n, uint8_t* out_dev,
                           int H, int W, irn_stream_t stream);
+
+/* ------------------------------------------------------------------------------------
+ * N1  exact JPEG decode on the device: bit-identical to np.asarray(Image.open(f).convert("RGB")) (PIL on libjpeg-turbo:
+ * islow IDCT, fancy chroma up-sampling), voc12/dataloader.py:101.  Our own kernels (csrc/jpeg_exact.cu); the arithmetic is
+ * oracle/jpeg.py's.  Supported: SOF0/SOF1 8-bit Huffman, one interleaved scan, 1 component (decoded to R=G=B) or Y Cb Cr with
+ * luma sampling 1x1 / 2x1 / 2x2 and chroma 1x1, optional DRI.  Anything else is -4 (unsupported); malformed or truncated
+ * headers are -1, found on the host before any launch.
+ *
+ * irn_jpeg_exact_inspect: host only, no device needed.  info[6] = H, W, components, luma h / v sampling, restart interval.
+ * irn_jpeg_exact_workspace_bytes: device workspace (256-byte aligned) and host staging bytes (pinned memory, so that the
+ *   upload is asynchronous) for these n streams.
+ * irn_jpeg_exact_decode: n host streams of any sizes; image i is written as uint8 RGB [H_i,W_i,3] at out_dev + out_offsets[i]
+ *   (out_offsets a HOST int64 [n]).  status_dev (device int32 [n]) is zeroed and then receives error bits for image i's
+ *   entropy-coded data (1 = stray marker, 2 = missing / surplus restart marker, 4 = invalid Huffman code, 8 = data ends early,
+ *   16 = AC run past the block); read it after the stream has reached this call.  host_staging must stay untouched until then.
+ * irn_jpeg_exact_set_timing / irn_jpeg_exact_last_ms: CUDA events between the stages of the next calls on this thread; last_ms
+ *   waits and returns the four durations of the last timed call (ms): unstuff, entropy decode, IDCT, up-sampling + colour.
+ */
+int irn_jpeg_exact_inspect(const uint8_t* data, size_t length, int* info);
+int irn_jpeg_exact_workspace_bytes(const uint8_t* const* data, const size_t* lengths, int n, size_t* device_bytes,
+                                   size_t* host_bytes);
+int irn_jpeg_exact_decode(const uint8_t* const* data, const size_t* lengths, int n, const int64_t* out_offsets, uint8_t* out_dev,
+                          int32_t* status_dev, void* workspace, size_t workspace_bytes, void* host_staging, size_t host_bytes,
+                          irn_stream_t stream);
+int irn_jpeg_exact_set_timing(int enable);
+int irn_jpeg_exact_last_ms(float* ms4);
 
 /* ------------------------------------------------------------------------------------
  * N3  fully connected CRF and the cam_to_ir_label step.  Replaces misc/imutils.py:156-170 (crf_inference_label: pydensecrf's

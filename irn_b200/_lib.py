@@ -74,6 +74,12 @@ SIGNATURES = {
     "irn_jpeg_decoder_destroy": (None, [c_void_p]),
     "irn_jpeg_image_size": (c_int, [c_void_p, c_void_p, c_size_t, _p_int, _p_int, _p_int]),
     "irn_jpeg_decode_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "irn_jpeg_exact_inspect": (c_int, [c_void_p, c_size_t, _p_int]),
+    "irn_jpeg_exact_workspace_bytes": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t)]),
+    "irn_jpeg_exact_decode": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t,
+                                      c_void_p]),
+    "irn_jpeg_exact_set_timing": (c_int, [c_int]),
+    "irn_jpeg_exact_last_ms": (c_int, [ctypes.POINTER(c_float)]),
     "irn_resize_ksize": (c_int, [c_int, c_int]),
     "irn_resize_coeffs": (c_int, [c_int, c_int, c_void_p, c_void_p]),
     "irn_normalize_lut": (c_int, [c_void_p, c_void_p, c_void_p]),

@@ -39,15 +39,17 @@ def collate_one(batch):
     """batch_size=1 collation like the reference's DataLoader, except that `size` stays a pair of python ints
     (torch's default collate makes it [tensor([H]), tensor([W])], which modern numpy can no longer use as a slice
     bound, step/make_sem_seg_labels.py:29,43)."""
-    jpeg = batch[0].pop("jpeg", None) if isinstance(batch[0], dict) else None
+    streams = {k: batch[0].pop(k) for k in JPEG_KINDS if isinstance(batch[0], dict) and k in batch[0]}
     out = default_collate(batch)
-    if jpeg is not None:
-        out["jpeg"] = torch.from_numpy(jpeg)        # variable-length byte stream: no batch dimension
+    for k, v in streams.items():
+        out[k] = torch.from_numpy(v)        # variable-length byte stream: no batch dimension
     out["size"] = (int(batch[0]["size"][0]), int(batch[0]["size"][1]))
     return out
 
 
 LOADER_CHUNK = 8
+# pack keys of JPEG file bytes: "jpeg" for nvJPEG (--device_jpeg True), "jpeg_exact" for the exact decoder (--device_jpeg exact)
+JPEG_KINDS = ("jpeg", "jpeg_exact")
 
 
 def collate_chunk(batch):
@@ -60,7 +62,7 @@ def collate_chunk(batch):
            "label": torch.stack([torch.as_tensor(b["label"]) for b in batch])}
     kinds, shapes, parts = [], [], []
     for b in batch:
-        k = "jpeg" if "jpeg" in b else "img_u8"
+        k = next((j for j in JPEG_KINDS if j in b), "img_u8")
         a = np.ascontiguousarray(b[k])
         kinds.append(k)
         shapes.append(tuple(a.shape))
@@ -82,7 +84,7 @@ def split_chunk(chunk):
         n = int(np.prod(shape))
         pack = {"name": [name], "size": chunk["sizes"][i], "label": chunk["label"][i:i + 1]}
         view = chunk["blob"][o:o + n]
-        pack[chunk["kinds"][i]] = view if chunk["kinds"][i] == "jpeg" else view.view((1,) + shape)
+        pack[chunk["kinds"][i]] = view if chunk["kinds"][i] in JPEG_KINDS else view.view((1,) + shape)
         o += n
         if "cam_blob" in chunk:
             cs = chunk["cam_shapes"][i]
@@ -109,9 +111,15 @@ def device_pyramid(args):
 
 
 def device_jpeg(args):
-    """--device_jpeg (default off): loader workers hand over the JPEG FILE BYTES, nvJPEG decodes them on the GPU
-    (irn_b200.jpeg).  Pixels differ from the host decoder's by a level or two: a throughput option, not a parity one."""
-    return bool(getattr(args, "device_jpeg", False)) and device_pyramid(args)
+    """--device_jpeg: which decoder turns JPEG file bytes into pixels on the GPU, or None (False, the default: the loader workers
+    decode on the host).  "exact": irn_b200.jpeg.ExactJpegDecoder, bit-identical to the host decoder; the workers ship the bytes of
+    the files it supports (jpeg.inspect) and decode the others, so a batch may mix both kinds; the steps that take raw images
+    (cam_to_ir_label) ship bytes too.  "nvjpeg" (True): nvJPEG, whose pixels differ from the host decoder's by a level or two: a
+    throughput option, not a parity one.  Either needs --device_pyramid."""
+    v = getattr(args, "device_jpeg", False)
+    if not v or not device_pyramid(args):
+        return None
+    return "exact" if str(v).lower() == "exact" else "nvjpeg"
 
 
 def step_batch(args):
@@ -126,7 +134,10 @@ PENDING_BOUND = 4
 
 
 def size_key(pack):
-    return (pack["size"], "jpeg" if "jpeg" in pack else tuple(pack["img_u8"].shape))
+    """Bucket key: exact-decoder bytes and host-decoded pixels of one size share a bucket (the same pixels either way)."""
+    if "jpeg" in pack:
+        return (pack["size"], "jpeg")
+    return (pack["size"], (1,) + tuple(pack["size"]) + (3,) if "jpeg_exact" in pack else tuple(pack["img_u8"].shape))
 
 
 class Batcher:
@@ -200,6 +211,7 @@ def make_dataset(args, list_path, scales, cam_dir=None, cam_field="cam", raw_ima
     if step_batch(args) == 1 or not (device_pyramid(args) or raw_images):
         cam_dir = None
     decode_only = True if raw_images else device_pyramid(args)
+    jpeg_mode = device_jpeg(args)
     if getattr(args, "synthetic", 0):
         # one id list for ALL steps (the reference reads --train_list in make_cam but --infer_list in the label steps; with
         # synthetic images the later steps must find the .npy files the first one wrote): --synthetic_list, else 2007_%06d
@@ -209,15 +221,29 @@ def make_dataset(args, list_path, scales, cam_dir=None, cam_field="cam", raw_ima
         return voc_data.SyntheticMSF(int(args.synthetic), scales=scales, name_list=names, decode_only=decode_only, cam_dir=cam_dir,
                                      cam_field=cam_field)
     return voc_data.VOC12ClassificationDatasetMSF(list_path, voc12_root=args.voc12_root, scales=scales, decode_only=decode_only,
-                                                  raw_jpeg=device_jpeg(args) and not raw_images, cam_dir=cam_dir, cam_field=cam_field)
+                                                  raw_jpeg=jpeg_mode if jpeg_mode == "exact" or not raw_images else None, cam_dir=cam_dir,
+                                                  cam_field=cam_field)
 
 
 _jpeg_decoders = {}
+_exact_decoders = {}
+
+
+def decode_exact(pack):
+    """A one-image pack holding exact-decoder bytes -> pack['img_u8'] uint8 [1,H,W,3] on the current device (the one-image loop)."""
+    if "jpeg_exact" in pack:
+        from ..jpeg import ExactJpegDecoder
+        dev = torch.device("cuda", torch.cuda.current_device())
+        if dev.index not in _exact_decoders:
+            _exact_decoders[dev.index] = ExactJpegDecoder(dev)
+        pack["img_u8"] = _exact_decoders[dev.index].decode([pack.pop("jpeg_exact")], names=pack["name"])
+    return pack
 
 
 def attach_pyramid(pack, scales):
     """Turn a decode-only item into what the reference's loader yields: pack['img'] = [1,2,3,h,w] per scale (a single
     tensor when there is one scale, voc12/dataloader.py:200-201), already on the current device."""
+    decode_exact(pack)
     if "jpeg" in pack:
         from ..jpeg import JpegDecoder
         dev = torch.device("cuda", torch.cuda.current_device())
@@ -249,6 +275,7 @@ class Writer:
         self.sem = threading.Semaphore(max_pending)
         self.file_sem = threading.Semaphore(max_files)
         self.futures, self.file_futures = [], []
+        self.checks = []        # callables the next batch job runs first, e.g. the status check of the batch's exact JPEG decode
         self._lock = threading.Lock()
         self._tls = threading.local()
 
@@ -276,12 +303,15 @@ class Writer:
     def submit(self, fn, *args):
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.device))
+        checks, self.checks = self.checks, []
         self.sem.acquire()
 
         def job():
             try:
                 with torch.cuda.device(self.device):
                     ev.synchronize()
+                    for c in checks:
+                        c()
                     fn(*args)
             finally:
                 self.sem.release()
@@ -337,6 +367,7 @@ class StepContext:
         self._pinned = {}
         self._flat = {"bufs": [None, None], "done": [None, None], "i": 0}     # pack_images' staging
         self._jpeg = None
+        self._exact = None
         self._copy_pool = ThreadPoolExecutor(max_workers=4)
         self.phase_seconds = {} if os.environ.get("IRN_STEP_PROFILE") else None     # host time per phase of the batch bodies
 
@@ -358,6 +389,9 @@ class StepContext:
         buffers per shape; a buffer is rewritten only after the upload that last read it has completed)."""
         if "jpeg" in packs[0]:       # --device_jpeg: file bytes -> nvJPEG -> uint8 [N,H,W,3] in HBM
             return self._jpeg_decoder().decode([p["jpeg"] for p in packs], size=packs[0]["size"])
+        if any("jpeg_exact" in p for p in packs):       # --device_jpeg exact: one size, so pack_images' layout is [N,H,W,3]
+            flat, sizes = self.pack_images(packs)
+            return flat.view((len(packs),) + tuple(sizes[0]) + (3,))
         N = len(packs)
         shape = (N,) + tuple(packs[0]["img_u8"].shape[1:])
         if shape not in self._pinned and len(self._pinned) >= 8:      # VOC has hundreds of image sizes: bound the pinned pool
@@ -390,7 +424,9 @@ class StepContext:
     def pack_images(self, packs):
         """The decoded images of a batch of any sizes as ONE flat device uint8 buffer, image i's [H_i,W_i,3] bytes back to back in
         pack order, and the list of (H_i, W_i).  Host images are staged through two alternating pinned buffers that grow to the
-        largest batch; with --device_jpeg every size group is decoded as one nvJPEG batch."""
+        largest batch; with --device_jpeg every size group is decoded as one nvJPEG batch.  With --device_jpeg exact the exact
+        decoder writes the packs that hold file bytes straight into the buffer, in one call whatever their sizes, and the host images
+        are copied in after them; the decode's status words are checked by the batch's writer job (Writer.checks)."""
         if "jpeg" in packs[0]:
             sizes = [tuple(p["size"]) for p in packs]
             groups = {}
@@ -402,6 +438,8 @@ class StepContext:
                 for k, i in enumerate(idx):
                     parts[i] = dec[k].reshape(-1)
             return (torch.cat(parts) if len(parts) > 1 else parts[0]), sizes
+        if any("jpeg_exact" in p for p in packs):
+            return self._pack_exact(packs)
         sizes = [(int(p["img_u8"].shape[1]), int(p["img_u8"].shape[2])) for p in packs]
         n = sum(3 * h * w for h, w in sizes)
         slot = self._flat
@@ -426,6 +464,32 @@ class StepContext:
         ev.record(torch.cuda.current_stream(self.device))
         slot["done"][k] = ev
         return dev, sizes
+
+    def _pack_exact(self, packs):
+        from ..jpeg import ExactJpegDecoder
+        if self._exact is None:
+            self._exact = ExactJpegDecoder(self.device)
+        sizes = [tuple(p["size"]) for p in packs]
+        offs = np.concatenate([[0], np.cumsum([3 * h * w for h, w in sizes])]).astype(np.int64)
+        out = torch.empty(int(offs[-1]), dtype=torch.uint8, device=self.device)
+        enc = [i for i, p in enumerate(packs) if "jpeg_exact" in p]
+        host = [i for i, p in enumerate(packs) if "jpeg_exact" not in p]
+        status = self._exact.decode_into([packs[i]["jpeg_exact"] for i in enc], offs[enc], out, [packs[i]["name"][0] for i in enc])
+        self.writer.checks.append(status.check)
+        if host:
+            flat, _ = self.pack_images([packs[i] for i in host])
+            o = 0
+            for i in host:
+                n = int(offs[i + 1] - offs[i])
+                out[int(offs[i]):int(offs[i + 1])].copy_(flat[o:o + n], non_blocking=True)
+                o += n
+        return out, sizes
+
+    def check_decoded(self):
+        """Run the pending exact-decode status checks now (for a batch body that has already waited for its results on the host)."""
+        checks, self.writer.checks = self.writer.checks, []
+        for c in checks:
+            c()
 
 
 def threaded_loader(shard, n_threads, prefetch):
@@ -471,7 +535,7 @@ def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragge
             model.cuda()
         if not batched:
             for it, pack in enumerate(loader):
-                per_image(model, attach_pyramid(pack, scales) if model is not None else pack, args)
+                per_image(model, attach_pyramid(pack, scales) if model is not None else decode_exact(pack), args)
                 progress(process_id, n_gpus, it, len(shard))
             return
         ctx = StepContext(model, args, torch.device("cuda", process_id), scales)

@@ -34,6 +34,7 @@ def ins_seg_batch(ctx, packs):
     edges, dps = ctx.pipe.irn_ragged_stage(x, sizes)
     strided = _common.to_device_list(ctx, cams)
     dets = ctx.pipe.instance_ragged_stage(strided, keys, edges, dps, sizes, float(args.ins_seg_bg_thres))
+    ctx.check_decoded()     # the detections are on the host: the stream has passed the batch's JPEG decode
     for name, det in zip(names, dets):
         if det is None:     # the reference's np.stack([]) raises for an image without any detection
             raise ValueError("need at least one array to stack (no instance detected in %s)" % name)

@@ -74,7 +74,8 @@ class VOC12ClassificationDatasetMSF(Dataset):
                  cls_labels_path="voc12/cls_labels.npy", decode_only=False, raw_jpeg=False, cam_dir=None, cam_field="cam"):
         self.cam_field = cam_field          # which map of the CAM dict the worker ships (attach_cam)
         self.decode_only = decode_only      # hand over the decoded uint8 image; the pyramid is built on the device
-        self.raw_jpeg = raw_jpeg            # hand over the FILE BYTES; nvJPEG decodes them on the device (irn_b200.jpeg)
+        # hand over the FILE BYTES, decoded on the device (irn_b200.jpeg): "exact" for the exact decoder, else (truthy) nvJPEG
+        self.raw_jpeg = raw_jpeg
         self.cam_dir = cam_dir              # label steps: the loader worker also reads the image's stored CAM dict (make_cam's .npy)
         self.img_name_list = load_img_name_list(img_name_list_path)
         self.voc12_root = voc12_root
@@ -88,7 +89,18 @@ class VOC12ClassificationDatasetMSF(Dataset):
 
     def __getitem__(self, idx):
         name_str = decode_int_filename(self.img_name_list[idx])
-        if self.raw_jpeg:
+        if self.raw_jpeg == "exact":
+            from .. import jpeg, _lib
+            with open(get_img_path(name_str, self.voc12_root), "rb") as f:
+                data = np.frombuffer(f.read(), dtype=np.uint8).copy()
+            try:
+                h, w = jpeg.inspect(data)[:2]
+            except _lib.IrnError:
+                pass        # not a stream the exact decoder takes (PNG stand-ins, progressive, CMYK, ...): decode on the host below
+            else:
+                return attach_cam({"name": name_str, "size": (h, w), "label": torch.from_numpy(self.label_list[idx]), "jpeg_exact": data},
+                                  self.cam_dir, self.cam_field)
+        elif self.raw_jpeg:
             path = get_img_path(name_str, self.voc12_root)
             with Image.open(path) as im:        # header only: the size decides the batch bucket
                 w, h = im.size

@@ -23,13 +23,18 @@ def _bool(v):
     return str(v).lower() in ("1", "true", "yes", "y")
 
 
+def _device_jpeg(v):
+    """--device_jpeg False (host decode) / True (nvJPEG) / exact (the exact device decoder)."""
+    return "exact" if str(v).lower() == "exact" else _bool(v)
+
+
 def _scales(v):
     return tuple(float(t) for t in str(v).split(","))
 
 
 # (flag, default, type) in the reference's order: environment, dataset, CAM, relation mining, IRNet, random walk, outputs
 FLAGS = [
-    ("num_workers", os.cpu_count() // 2, int), ("voc12_root", "", str), ("synthetic", 0, int), ("synthetic_list", "", str), ("device_pyramid", True, _bool), ("device_jpeg", False, _bool),
+    ("num_workers", os.cpu_count() // 2, int), ("voc12_root", "", str), ("synthetic", 0, int), ("synthetic_list", "", str), ("device_pyramid", True, _bool), ("device_jpeg", False, _device_jpeg),
     ("step_batch", 32, int), ("loader_threads", False, _bool),
     ("train_list", "voc12/train_aug.txt", str), ("val_list", "voc12/val.txt", str), ("infer_list", "voc12/train.txt", str),
     ("chainer_eval_set", "train", str),
