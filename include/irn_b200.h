@@ -339,21 +339,6 @@ int irn_resize_ragged_forward(const uint8_t* img_u8, size_t img_bytes, const int
                               void* workspace, size_t workspace_bytes, irn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------
- * N1  JPEG decode on the device (nvJPEG, loaded with dlopen at decoder creation) in place of `imageio.imread` in
- * VOC12ClassificationDatasetMSF.__getitem__ (voc12/dataloader.py:189): n JPEG streams of one size (host pointers) ->
- * uint8 [n,H,W,3] RGB in HBM, the input layout of irn_resize_forward.  backend 0 = nvJPEG's default GPU-assisted decoder,
- * 1 = the hardware JPEG engine when the device has one (falls back to 0; irn_jpeg_decoder_backend tells).  NOT bit-identical
- * to libjpeg-turbo (+-1..2 levels): a throughput option; parity runs decode on the host or with irn_jpeg_exact_* below.
- */
-typedef struct irn_jpeg irn_jpeg;
-int irn_jpeg_decoder_create(int backend, irn_jpeg** out);
-int irn_jpeg_decoder_backend(const irn_jpeg* decoder);
-void irn_jpeg_decoder_destroy(irn_jpeg* decoder);
-int irn_jpeg_image_size(irn_jpeg* decoder, const uint8_t* data, size_t length, int* H, int* W, int* n_components);
-int irn_jpeg_decode_batch(irn_jpeg* decoder, const uint8_t* const* data, const size_t* lengths, int n, uint8_t* out_dev,
-                          int H, int W, irn_stream_t stream);
-
-/* ------------------------------------------------------------------------------------
  * N1  exact JPEG decode on the device: bit-identical to np.asarray(Image.open(f).convert("RGB")) (PIL on libjpeg-turbo:
  * islow IDCT, fancy chroma up-sampling), voc12/dataloader.py:101.  Our own kernels (csrc/jpeg_exact.cu); the arithmetic is
  * oracle/jpeg.py's.  Supported: SOF0/SOF1 8-bit Huffman, one interleaved scan, 1 component (decoded to R=G=B) or Y Cb Cr with

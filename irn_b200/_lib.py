@@ -69,11 +69,6 @@ SIGNATURES = {
     "irn_segment_masks": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "irn_rw_labels": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p,
                               c_void_p, c_void_p, c_void_p]),
-    "irn_jpeg_decoder_create": (c_int, [c_int, ctypes.POINTER(c_void_p)]),
-    "irn_jpeg_decoder_backend": (c_int, [c_void_p]),
-    "irn_jpeg_decoder_destroy": (None, [c_void_p]),
-    "irn_jpeg_image_size": (c_int, [c_void_p, c_void_p, c_size_t, _p_int, _p_int, _p_int]),
-    "irn_jpeg_decode_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]),
     "irn_jpeg_exact_inspect": (c_int, [c_void_p, c_size_t, _p_int]),
     "irn_jpeg_exact_workspace_bytes": (c_int, [c_void_p, c_void_p, c_int, ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t)]),
     "irn_jpeg_exact_decode": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t,

@@ -1,11 +1,8 @@
-"""N1: JPEG decode on the device in place of the loader's host decode (voc12/dataloader.py:101), two decoders:
+"""N1: JPEG decode on the device in place of the loader's host decode (voc12/dataloader.py:101).
 
-``ExactJpegDecoder`` (``--device_jpeg exact``): our own kernels (csrc/jpeg_exact.cu, include/irn_b200.h irn_jpeg_exact_*), bit-identical
+``ExactJpegDecoder`` (``--device_jpeg True``): our own kernels (csrc/jpeg_exact.cu, include/irn_b200.h irn_jpeg_exact_*), bit-identical
 to ``np.asarray(Image.open(f).convert("RGB"))`` on libjpeg-turbo for the baseline streams ``inspect`` accepts; images of any sizes in
-one call.
-
-``JpegDecoder`` (``--device_jpeg True``): nvJPEG through the C ABI (irn_jpeg_*).  A throughput option: nvJPEG's IDCT / chroma
-up-sampling differ from libjpeg-turbo's, so its pixels are not bit-identical to the reference's loader."""
+one call."""
 import ctypes
 from collections import deque
 
@@ -13,47 +10,6 @@ import numpy as np
 import torch
 
 from . import _lib
-
-
-class JpegDecoder:
-    def __init__(self, device, backend="hardware"):
-        self.device = torch.device(device)
-        h = ctypes.c_void_p()
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().irn_jpeg_decoder_create(1 if backend == "hardware" else 0, ctypes.byref(h)), "irn_jpeg_decoder_create")
-        self.handle = h
-        self.backend = "hardware" if _lib.lib().irn_jpeg_decoder_backend(h) == 1 else "default"
-
-    def __del__(self):
-        try:
-            if self.handle:
-                _lib.lib().irn_jpeg_decoder_destroy(self.handle)
-        except Exception:
-            pass
-
-    def image_size(self, data):
-        buf = np.frombuffer(data, dtype=np.uint8)
-        H, W, C = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
-        _lib.check(_lib.lib().irn_jpeg_image_size(self.handle, buf.ctypes.data, buf.size, ctypes.byref(H), ctypes.byref(W), ctypes.byref(C)),
-                   "irn_jpeg_image_size")
-        return H.value, W.value
-
-    def decode(self, streams, size=None, out=None):
-        """streams: sequence of bytes-like / uint8 arrays / uint8 CPU tensors holding JPEG files of ONE image size.
-        Returns uint8 cuda [n,H,W,3] (RGB), enqueued on the current stream."""
-        bufs = [s.numpy() if isinstance(s, torch.Tensor) else np.frombuffer(s, dtype=np.uint8) for s in streams]
-        n = len(bufs)
-        if n == 0:
-            raise _lib.IrnError("JpegDecoder.decode: empty batch")
-        H, W = size if size is not None else self.image_size(bufs[0])
-        if out is None:
-            out = torch.empty((n, H, W, 3), dtype=torch.uint8, device=self.device)
-        ptrs = (ctypes.c_void_p * n)(*[b.ctypes.data for b in bufs])
-        lens = (ctypes.c_size_t * n)(*[b.size for b in bufs])
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().irn_jpeg_decode_batch(self.handle, ptrs, lens, n, _lib.ptr(out), int(H), int(W), _lib.stream_ptr()),
-                       "irn_jpeg_decode_batch")
-        return out
 
 
 class UnsupportedJpeg(_lib.IrnError):

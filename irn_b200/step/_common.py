@@ -39,17 +39,15 @@ def collate_one(batch):
     """batch_size=1 collation like the reference's DataLoader, except that `size` stays a pair of python ints
     (torch's default collate makes it [tensor([H]), tensor([W])], which modern numpy can no longer use as a slice
     bound, step/make_sem_seg_labels.py:29,43)."""
-    streams = {k: batch[0].pop(k) for k in JPEG_KINDS if isinstance(batch[0], dict) and k in batch[0]}
+    stream = batch[0].pop("jpeg_exact", None) if isinstance(batch[0], dict) else None
     out = default_collate(batch)
-    for k, v in streams.items():
-        out[k] = torch.from_numpy(v)        # variable-length byte stream: no batch dimension
+    if stream is not None:
+        out["jpeg_exact"] = torch.from_numpy(stream)        # variable-length byte stream: no batch dimension
     out["size"] = (int(batch[0]["size"][0]), int(batch[0]["size"][1]))
     return out
 
 
 LOADER_CHUNK = 8
-# pack keys of JPEG file bytes: "jpeg" for nvJPEG (--device_jpeg True), "jpeg_exact" for the exact decoder (--device_jpeg exact)
-JPEG_KINDS = ("jpeg", "jpeg_exact")
 
 
 def collate_chunk(batch):
@@ -62,7 +60,7 @@ def collate_chunk(batch):
            "label": torch.stack([torch.as_tensor(b["label"]) for b in batch])}
     kinds, shapes, parts = [], [], []
     for b in batch:
-        k = next((j for j in JPEG_KINDS if j in b), "img_u8")
+        k = "jpeg_exact" if "jpeg_exact" in b else "img_u8"
         a = np.ascontiguousarray(b[k])
         kinds.append(k)
         shapes.append(tuple(a.shape))
@@ -84,7 +82,7 @@ def split_chunk(chunk):
         n = int(np.prod(shape))
         pack = {"name": [name], "size": chunk["sizes"][i], "label": chunk["label"][i:i + 1]}
         view = chunk["blob"][o:o + n]
-        pack[chunk["kinds"][i]] = view if chunk["kinds"][i] in JPEG_KINDS else view.view((1,) + shape)
+        pack[chunk["kinds"][i]] = view if chunk["kinds"][i] == "jpeg_exact" else view.view((1,) + shape)
         o += n
         if "cam_blob" in chunk:
             cs = chunk["cam_shapes"][i]
@@ -111,15 +109,11 @@ def device_pyramid(args):
 
 
 def device_jpeg(args):
-    """--device_jpeg: which decoder turns JPEG file bytes into pixels on the GPU, or None (False, the default: the loader workers
-    decode on the host).  "exact": irn_b200.jpeg.ExactJpegDecoder, bit-identical to the host decoder; the workers ship the bytes of
-    the files it supports (jpeg.inspect) and decode the others, so a batch may mix both kinds; the steps that take raw images
-    (cam_to_ir_label) ship bytes too.  "nvjpeg" (True): nvJPEG, whose pixels differ from the host decoder's by a level or two: a
-    throughput option, not a parity one.  Either needs --device_pyramid."""
-    v = getattr(args, "device_jpeg", False)
-    if not v or not device_pyramid(args):
-        return None
-    return "exact" if str(v).lower() == "exact" else "nvjpeg"
+    """--device_jpeg (True or "exact"; False, the default, has the loader workers decode on the host): JPEG file bytes are decoded
+    on the GPU by irn_b200.jpeg.ExactJpegDecoder, bit-identical to the host decoder; the workers ship the bytes of the files it
+    supports (jpeg.inspect) and decode the others, so a batch may mix both kinds; the steps that take raw images (cam_to_ir_label)
+    ship bytes too.  Needs --device_pyramid."""
+    return bool(getattr(args, "device_jpeg", False)) and device_pyramid(args)
 
 
 def step_batch(args):
@@ -134,10 +128,8 @@ PENDING_BOUND = 4
 
 
 def size_key(pack):
-    """Bucket key: exact-decoder bytes and host-decoded pixels of one size share a bucket (the same pixels either way)."""
-    if "jpeg" in pack:
-        return (pack["size"], "jpeg")
-    return (pack["size"], (1,) + tuple(pack["size"]) + (3,) if "jpeg_exact" in pack else tuple(pack["img_u8"].shape))
+    """Bucket key (H, W): exact-decoder bytes and host-decoded pixels of one size share a bucket (the same pixels either way)."""
+    return tuple(pack["size"])
 
 
 class Batcher:
@@ -174,14 +166,14 @@ class Batcher:
     def _flush(self, key):
         packs = self.buckets.pop(key)
         if self.riders and len(packs) < self.bsz:
-            packs += self._take_riders(key[0], self.bsz - len(packs))
+            packs += self._take_riders(key, self.bsz - len(packs))
         self.pending -= len(packs)
         self.per_batch(self.ctx, packs)
 
     def _take_riders(self, size, n):
         """Up to n pending items of sizes that fit inside `size` = (H, W) with at least half its area, the smallest buckets first."""
         H, W = size
-        fits = [k for k in self.buckets if k[0][0] <= H and k[0][1] <= W and 2 * k[0][0] * k[0][1] >= H * W]
+        fits = [k for k in self.buckets if k[0] <= H and k[1] <= W and 2 * k[0] * k[1] >= H * W]
         out = []
         for k in sorted(fits, key=lambda k: len(self.buckets[k])):
             b = self.buckets[k]
@@ -197,7 +189,7 @@ class Batcher:
     def finish(self):
         if self.riders:     # the largest images first: every other bucket may still ride with them
             while self.buckets:
-                self._flush(max(self.buckets, key=lambda k: (k[0][0] * k[0][1], len(self.buckets[k]))))
+                self._flush(max(self.buckets, key=lambda k: (k[0] * k[1], len(self.buckets[k]))))
             return
         for key in list(self.buckets):
             self._flush(key)
@@ -211,7 +203,6 @@ def make_dataset(args, list_path, scales, cam_dir=None, cam_field="cam", raw_ima
     if step_batch(args) == 1 or not (device_pyramid(args) or raw_images):
         cam_dir = None
     decode_only = True if raw_images else device_pyramid(args)
-    jpeg_mode = device_jpeg(args)
     if getattr(args, "synthetic", 0):
         # one id list for ALL steps (the reference reads --train_list in make_cam but --infer_list in the label steps; with
         # synthetic images the later steps must find the .npy files the first one wrote): --synthetic_list, else 2007_%06d
@@ -221,11 +212,9 @@ def make_dataset(args, list_path, scales, cam_dir=None, cam_field="cam", raw_ima
         return voc_data.SyntheticMSF(int(args.synthetic), scales=scales, name_list=names, decode_only=decode_only, cam_dir=cam_dir,
                                      cam_field=cam_field)
     return voc_data.VOC12ClassificationDatasetMSF(list_path, voc12_root=args.voc12_root, scales=scales, decode_only=decode_only,
-                                                  raw_jpeg=jpeg_mode if jpeg_mode == "exact" or not raw_images else None, cam_dir=cam_dir,
-                                                  cam_field=cam_field)
+                                                  raw_jpeg=device_jpeg(args), cam_dir=cam_dir, cam_field=cam_field)
 
 
-_jpeg_decoders = {}
 _exact_decoders = {}
 
 
@@ -244,12 +233,6 @@ def attach_pyramid(pack, scales):
     """Turn a decode-only item into what the reference's loader yields: pack['img'] = [1,2,3,h,w] per scale (a single
     tensor when there is one scale, voc12/dataloader.py:200-201), already on the current device."""
     decode_exact(pack)
-    if "jpeg" in pack:
-        from ..jpeg import JpegDecoder
-        dev = torch.device("cuda", torch.cuda.current_device())
-        if dev.index not in _jpeg_decoders:
-            _jpeg_decoders[dev.index] = JpegDecoder(dev)
-        pack["img_u8"] = _jpeg_decoders[dev.index].decode([pack["jpeg"]], size=pack["size"])
     if "img_u8" not in pack:
         return pack
     pyr = preprocess.msf_batch(pack["img_u8"].cuda(non_blocking=True), scales)
@@ -364,9 +347,7 @@ class StepContext:
             self.pipe = PseudoLabelPipeline(model if is_cam else None, None if is_cam else model, device, self.scales,
                                             beta=float(getattr(args, "beta", 10)), exp_times=int(getattr(args, "exp_times", 8)))
         self.writer = Writer(device)
-        self._pinned = {}
         self._flat = {"bufs": [None, None], "done": [None, None], "i": 0}     # pack_images' staging
-        self._jpeg = None
         self._exact = None
         self._copy_pool = ThreadPoolExecutor(max_workers=4)
         self.phase_seconds = {} if os.environ.get("IRN_STEP_PROFILE") else None     # host time per phase of the batch bodies
@@ -384,60 +365,13 @@ class StepContext:
         finally:
             self.phase_seconds[name] = self.phase_seconds.get(name, 0.0) + time.perf_counter() - t
 
-    def stack_images(self, packs):
-        """The decoded images of a bucket as one device uint8 [N,H,W,3], staged through pinned host memory (two alternating
-        buffers per shape; a buffer is rewritten only after the upload that last read it has completed)."""
-        if "jpeg" in packs[0]:       # --device_jpeg: file bytes -> nvJPEG -> uint8 [N,H,W,3] in HBM
-            return self._jpeg_decoder().decode([p["jpeg"] for p in packs], size=packs[0]["size"])
-        if any("jpeg_exact" in p for p in packs):       # --device_jpeg exact: one size, so pack_images' layout is [N,H,W,3]
-            flat, sizes = self.pack_images(packs)
-            return flat.view((len(packs),) + tuple(sizes[0]) + (3,))
-        N = len(packs)
-        shape = (N,) + tuple(packs[0]["img_u8"].shape[1:])
-        if shape not in self._pinned and len(self._pinned) >= 8:      # VOC has hundreds of image sizes: bound the pinned pool
-            torch.cuda.current_stream(self.device).synchronize()
-            self._pinned.clear()
-        slot = self._pinned.setdefault(shape, {"bufs": [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(2)],
-                                               "done": [None, None], "i": 0})
-        k = slot["i"]
-        slot["i"] ^= 1
-        if slot["done"][k] is not None:
-            slot["done"][k].synchronize()
-        buf = slot["bufs"][k]
-        if N >= 16:      # 50 MB per bucket of 64: a few threads (copy_ releases the GIL) instead of ~20 ms of the loop's only thread
-            list(self._copy_pool.map(lambda i: buf[i].copy_(packs[i]["img_u8"][0]), range(N)))
-        else:
-            for i, p in enumerate(packs):
-                buf[i].copy_(p["img_u8"][0])
-        dev = buf.to(self.device, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(self.device))
-        slot["done"][k] = ev
-        return dev
-
-    def _jpeg_decoder(self):
-        if self._jpeg is None:
-            from ..jpeg import JpegDecoder
-            self._jpeg = JpegDecoder(self.device)
-        return self._jpeg
-
     def pack_images(self, packs):
         """The decoded images of a batch of any sizes as ONE flat device uint8 buffer, image i's [H_i,W_i,3] bytes back to back in
-        pack order, and the list of (H_i, W_i).  Host images are staged through two alternating pinned buffers that grow to the
-        largest batch; with --device_jpeg every size group is decoded as one nvJPEG batch.  With --device_jpeg exact the exact
-        decoder writes the packs that hold file bytes straight into the buffer, in one call whatever their sizes, and the host images
-        are copied in after them; the decode's status words are checked by the batch's writer job (Writer.checks)."""
-        if "jpeg" in packs[0]:
-            sizes = [tuple(p["size"]) for p in packs]
-            groups = {}
-            for i, s in enumerate(sizes):
-                groups.setdefault(s, []).append(i)
-            parts = [None] * len(packs)
-            for s, idx in groups.items():
-                dec = self._jpeg_decoder().decode([packs[i]["jpeg"] for i in idx], size=s)
-                for k, i in enumerate(idx):
-                    parts[i] = dec[k].reshape(-1)
-            return (torch.cat(parts) if len(parts) > 1 else parts[0]), sizes
+        pack order, and the list of (H_i, W_i); for a batch of one size the buffer is the [N,H,W,3] stack.  Host images are staged
+        through two alternating pinned buffers that grow to the largest batch (a buffer is rewritten only after the upload that last
+        read it has completed).  With --device_jpeg the exact decoder writes the packs that hold file bytes straight into the buffer,
+        in one call whatever their sizes, and the host images are copied in after them; the decode's status words are checked by the
+        batch's writer job (Writer.checks)."""
         if any("jpeg_exact" in p for p in packs):
             return self._pack_exact(packs)
         sizes = [(int(p["img_u8"].shape[1]), int(p["img_u8"].shape[2])) for p in packs]
@@ -492,28 +426,6 @@ class StepContext:
             c()
 
 
-def threaded_loader(shard, n_threads, prefetch):
-    """Items of `shard` in order, collated like the batch-size-1 DataLoader, produced by a thread pool instead of forked worker
-    processes: PIL's JPEG decoder and the file reads release the GIL, and a thread hands its arrays over without the
-    shared-memory copy -- and without the ~1 s it takes to fork a dozen workers off a process that holds a CUDA context.  Usually
-    slower than the forked workers (the unpickling of the CAM dicts, numpy copies and collation serialise on the GIL), so it is
-    opt-in (--loader_threads True) and kept for hosts where fork is the problem."""
-    from collections import deque
-    n = len(shard)
-    with ThreadPoolExecutor(max_workers=max(1, n_threads)) as pool:
-        pending = deque()
-        nxt = 0
-        while nxt < n and len(pending) < prefetch:
-            pending.append(pool.submit(shard.__getitem__, nxt))
-            nxt += 1
-        while pending:
-            item = pending.popleft().result()
-            if nxt < n:
-                pending.append(pool.submit(shard.__getitem__, nxt))
-                nxt += 1
-            yield collate_one([item])
-
-
 def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragged=False, riders=False):
     """One GPU's share: the reference's `_work(process_id, model, dataset, args)` signature and loop order
     (step/make_cam.py:16-59), with the per-image / per-batch body supplied by the step.  model None: a step without a network
@@ -539,9 +451,6 @@ def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragge
                 progress(process_id, n_gpus, it, len(shard))
             return
         ctx = StepContext(model, args, torch.device("cuda", process_id), scales)
-        chunked = True
-        if getattr(args, "loader_threads", False):     # slower than forked workers (GIL): off
-            loader, chunked = threaded_loader(shard, max(2, args.num_workers // n_gpus), prefetch=2 * bsz), False
         batcher = Batcher(ctx, per_batch, bsz, ragged, riders)
         prof = os.environ.get("IRN_STEP_PROFILE")          # host-side time split of the loop (development aid), printed to stderr
         t_load = t_body = 0.0
@@ -551,7 +460,7 @@ def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragge
             for msg in loader:
                 t_now = time.perf_counter()
                 t_load += t_now - t_prev
-                for pack in (split_chunk(msg) if chunked else (msg,)):
+                for pack in split_chunk(msg):
                     batcher.add(pack)
                     progress(process_id, n_gpus, it, len(shard))
                     it += 1

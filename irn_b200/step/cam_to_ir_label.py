@@ -40,8 +40,9 @@ def ir_label_batch(ctx, packs):
     names = [voc_data.decode_int_filename(p["name"][0]) for p in packs]
     with ctx.phase("cam dicts"):
         keys, high = _common.load_cam_dicts(ctx, packs, names, args.cam_out_dir, field="high_res")
-    with ctx.phase("stack + upload images"):
-        x = ctx.stack_images(packs)
+    with ctx.phase("pack + upload images"):
+        flat, sizes = ctx.pack_images(packs)
+        x = flat.view((len(packs),) + sizes[0] + (3,))
     with ctx.phase("crf"):
         conf = crf.ir_labels(x, [torch.as_tensor(h) for h in high], keys, args.conf_fg_thres, args.conf_bg_thres)
     with ctx.phase("hand to writer"):

@@ -37,16 +37,14 @@ def cam_batch(ctx, packs):
     with smaller images (_common.Batcher), which run on the bucket's canvas (cam_ragged_stage)."""
     args = ctx.args
     labels = torch.cat([p["label"] for p in packs], 0)
-    if len({_common.size_key(p) for p in packs}) > 1:
-        with ctx.phase("pack + upload images"):
-            flat, sizes = ctx.pack_images(packs)
+    with ctx.phase("pack + upload images"):
+        flat, sizes = ctx.pack_images(packs)
+    if len(set(sizes)) > 1:
         with ctx.phase("ragged pyramids + cam forward + merge (issue)"):
             keys, strided, highres = ctx.pipe.cam_ragged_stage(flat, sizes, labels, want_highres=True, scales=ctx.scales)
     else:
-        with ctx.phase("stack + upload images"):
-            x = ctx.stack_images(packs)
         with ctx.phase("pyramids + cam forward + merge (issue)"):
-            xs = ctx.pipe.pyramids(x, ctx.scales)
+            xs = ctx.pipe.pyramids(flat.view((len(packs),) + sizes[0] + (3,)), ctx.scales)
             keys, strided, highres = ctx.pipe.cam_stage(xs, labels, packs[0]["size"], want_highres=True, scales=ctx.scales)
     with ctx.phase("hand to writer"):
         ctx.writer.submit(_save, ctx, [p["name"][0] for p in packs], keys, strided, highres, args.cam_out_dir)

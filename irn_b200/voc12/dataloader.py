@@ -74,8 +74,7 @@ class VOC12ClassificationDatasetMSF(Dataset):
                  cls_labels_path="voc12/cls_labels.npy", decode_only=False, raw_jpeg=False, cam_dir=None, cam_field="cam"):
         self.cam_field = cam_field          # which map of the CAM dict the worker ships (attach_cam)
         self.decode_only = decode_only      # hand over the decoded uint8 image; the pyramid is built on the device
-        # hand over the FILE BYTES, decoded on the device (irn_b200.jpeg): "exact" for the exact decoder, else (truthy) nvJPEG
-        self.raw_jpeg = raw_jpeg
+        self.raw_jpeg = raw_jpeg            # hand over the FILE BYTES; the exact decoder decodes them on the device (irn_b200.jpeg)
         self.cam_dir = cam_dir              # label steps: the loader worker also reads the image's stored CAM dict (make_cam's .npy)
         self.img_name_list = load_img_name_list(img_name_list_path)
         self.voc12_root = voc12_root
@@ -89,7 +88,7 @@ class VOC12ClassificationDatasetMSF(Dataset):
 
     def __getitem__(self, idx):
         name_str = decode_int_filename(self.img_name_list[idx])
-        if self.raw_jpeg == "exact":
+        if self.raw_jpeg:
             from .. import jpeg, _lib
             with open(get_img_path(name_str, self.voc12_root), "rb") as f:
                 data = np.frombuffer(f.read(), dtype=np.uint8).copy()
@@ -100,16 +99,6 @@ class VOC12ClassificationDatasetMSF(Dataset):
             else:
                 return attach_cam({"name": name_str, "size": (h, w), "label": torch.from_numpy(self.label_list[idx]), "jpeg_exact": data},
                                   self.cam_dir, self.cam_field)
-        elif self.raw_jpeg:
-            path = get_img_path(name_str, self.voc12_root)
-            with Image.open(path) as im:        # header only: the size decides the batch bucket
-                w, h = im.size
-                is_jpeg = im.format == "JPEG" and im.mode == "RGB"
-            if is_jpeg:
-                with open(path, "rb") as f:
-                    data = np.frombuffer(f.read(), dtype=np.uint8).copy()
-                return attach_cam({"name": name_str, "size": (h, w), "label": torch.from_numpy(self.label_list[idx]), "jpeg": data}, self.cam_dir, self.cam_field)
-            # not a 3-component JPEG (grey-scale / PNG stand-ins): decode on the host like the reference
         img = np.asarray(Image.open(get_img_path(name_str, self.voc12_root)).convert("RGB"))
         out = {"name": name_str, "size": (img.shape[0], img.shape[1]), "label": torch.from_numpy(self.label_list[idx])}
         if self.decode_only:

@@ -11,7 +11,8 @@ Differences: --cam_network / --irn_network default to the irn_b200 modules; flag
 (--beta, --exp_times, --*_bg_thres, --*_pass) are parsed; --synthetic N runs on N seeded synthetic images instead of VOC
 (--synthetic_list names them); --step_batch N images are processed together (of
 any sizes in make_sem_seg_labels / make_ins_seg_labels, of one size in cam_to_ir_label, of one size in make_cam except for buckets
-flushed before they fill, which take smaller images along; 1 = the reference's loop).
+flushed before they fill, which take smaller images along; 1 = the reference's loop); --device_jpeg True decodes the JPEG
+files the exact device decoder supports on the GPU, bit-identical to the host decode, so every output file is the same.
 """
 import argparse
 import os
@@ -24,8 +25,8 @@ def _bool(v):
 
 
 def _device_jpeg(v):
-    """--device_jpeg False (host decode) / True (nvJPEG) / exact (the exact device decoder)."""
-    return "exact" if str(v).lower() == "exact" else _bool(v)
+    """--device_jpeg False (host decode) / True (the exact device decoder); `exact` is accepted as a spelling of True."""
+    return str(v).lower() == "exact" or _bool(v)
 
 
 def _scales(v):
@@ -35,7 +36,7 @@ def _scales(v):
 # (flag, default, type) in the reference's order: environment, dataset, CAM, relation mining, IRNet, random walk, outputs
 FLAGS = [
     ("num_workers", os.cpu_count() // 2, int), ("voc12_root", "", str), ("synthetic", 0, int), ("synthetic_list", "", str), ("device_pyramid", True, _bool), ("device_jpeg", False, _device_jpeg),
-    ("step_batch", 32, int), ("loader_threads", False, _bool),
+    ("step_batch", 32, int),
     ("train_list", "voc12/train_aug.txt", str), ("val_list", "voc12/val.txt", str), ("infer_list", "voc12/train.txt", str),
     ("chainer_eval_set", "train", str),
     ("cam_network", "irn_b200.cam", str), ("cam_crop_size", 512, int), ("cam_batch_size", 16, int), ("cam_num_epoches", 5, int),

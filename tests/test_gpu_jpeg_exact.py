@@ -186,7 +186,7 @@ def test_steps_write_the_same_files_as_host_decode(voc_tree):
     _same_png(h.sem_seg_out_dir, e.sem_seg_out_dir, ids)
     _same_npy(h.ins_seg_out_dir, e.ins_seg_out_dir, ids)
     _same_png(h.ir_label_out_dir, e.ir_label_out_dir, ids)
-    # a one-size list (full buckets, stack_images), and the one-image loop of cam_to_ir_label (reads e's CAMs)
+    # a one-size list (full buckets, the one-size CAM stage), and the one-image loop of cam_to_ir_label (reads e's CAMs)
     one_runs = [_args(root, tag + "_one", "one.txt", device_jpeg=dj) for tag, dj in (("host", False), ("exact", "exact"))]
     for a in one_runs:
         make_cam.run(a)

@@ -123,19 +123,7 @@ def test_loader_attaches_stored_cams(tmp_path):
     assert _common.make_dataset(args, "x", (1.0,), cam_dir=str(cam_dir)).cam_dir == str(cam_dir)
 
 
-def test_threaded_loader_matches_dataloader_order():
-    """Batched mode's thread-pool loader: same items, same order, same batch-1 collation as the DataLoader it replaces."""
-    ds = dl.SyntheticMSF(7, size=(24, 32), scales=(1.0,), decode_only=True)
-    shard = torchutils.split_dataset(ds, 2)[1]
-    got = list(_common.threaded_loader(shard, 3, prefetch=4))
-    assert [p["name"] for p in got] == [["2007_%06d" % i] for i in (1, 3, 5)]
-    from torch.utils.data import DataLoader
-    ref = list(DataLoader(shard, shuffle=False, num_workers=0, collate_fn=_common.collate_one))
-    for a, b in zip(got, ref):
-        assert a["size"] == b["size"] and torch.equal(a["img_u8"], b["img_u8"]) and torch.equal(a["label"], b["label"])
-
-
-def test_chunked_messages_split_back_into_batch1_packs(tmp_path):
+def test_chunked_messages_with_exact_bytes_split_back_into_batch1_packs(tmp_path):
     """Batched mode ships LOADER_CHUNK items per worker message (step/_common.collate_chunk: one flat tensor for the pixels / JPEG
     bytes, one for the stored CAMs); split_chunk must give back exactly the packs of the batch-size-1 collation, in order,
     including ragged items (different image sizes, different K, a JPEG byte stream next to decoded pixels)."""
@@ -148,7 +136,7 @@ def test_chunked_messages_split_back_into_batch1_packs(tmp_path):
         item = {"name": "2007_%06d" % i, "size": (h, w), "label": torch.from_numpy(rng.rand(20).astype(np.float32)),
                 "cam_keys": torch.arange(k, dtype=torch.int64) + i, "cam": torch.from_numpy(rng.rand(k, h // 4, w // 4).astype(np.float32))}
         if i == 1:
-            item["jpeg"] = rng.randint(0, 255, 777).astype(np.uint8)
+            item["jpeg_exact"] = rng.randint(0, 255, 777).astype(np.uint8)
         else:
             item["img_u8"] = rng.randint(0, 255, (h, w, 3)).astype(np.uint8)
         items.append(item)
@@ -158,7 +146,7 @@ def test_chunked_messages_split_back_into_batch1_packs(tmp_path):
         ref = _common.collate_one([dict(it)])
         assert set(p) == set(ref)
         assert p["name"] == ref["name"] and p["size"] == ref["size"]
-        for k in ("label", "cam", "cam_keys", "img_u8", "jpeg"):
+        for k in ("label", "cam", "cam_keys", "img_u8", "jpeg_exact"):
             if k in ref:
                 assert p[k].shape == ref[k].shape and p[k].dtype == ref[k].dtype and torch.equal(p[k], ref[k]), k
     # through a real DataLoader with workers, over a stride shard: same items, same order as the batch-1 loader

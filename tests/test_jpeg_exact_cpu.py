@@ -1,5 +1,5 @@
 """The exact JPEG decoder's host side: its oracle (oracle/jpeg.py) against PIL bit for bit, the header inspection that decides which
-streams the device decoder takes (irn_b200.jpeg.inspect, the C ABI's irn_jpeg_exact_inspect), --device_jpeg exact parsing and the
+streams the device decoder takes (irn_b200.jpeg.inspect, the C ABI's irn_jpeg_exact_inspect), --device_jpeg parsing and the
 loader's routing of file bytes vs host-decoded pixels."""
 import io
 import os
@@ -85,19 +85,20 @@ def test_inspect_classifies_streams():
             oracle_jpeg.inspect(data)
 
 
-def test_device_jpeg_flag_parses():
+def test_device_jpeg_flag_parses_to_a_bool():
     import run_sample
     from irn_b200.step import _common
-    for v, want, mode in (("exact", "exact", "exact"), ("EXACT", "exact", "exact"), ("True", True, "nvjpeg"), ("False", False, None)):
+    for v, want in (("exact", True), ("EXACT", True), ("True", True), ("False", False)):
         a = run_sample.parse(["--device_jpeg", v])
-        assert a.device_jpeg == want
-        assert _common.device_jpeg(a) == mode
+        assert a.device_jpeg is want
+        assert _common.device_jpeg(a) is want
     assert run_sample.parse([]).device_jpeg is False
-    assert _common.device_jpeg(types.SimpleNamespace(device_jpeg="exact", device_pyramid=False)) is None
+    assert _common.device_jpeg(types.SimpleNamespace(device_jpeg="exact", device_pyramid=True)) is True
+    assert _common.device_jpeg(types.SimpleNamespace(device_jpeg="exact", device_pyramid=False)) is False
 
 
-def test_loader_routes_bytes_and_host_pixels(tmp_path):
-    """--device_jpeg exact: the worker ships the bytes of a file the exact decoder takes and decodes the others (PNG stand-in,
+def test_loader_routes_exact_bytes_and_host_pixels(tmp_path):
+    """--device_jpeg: the worker ships the bytes of a file the exact decoder takes and decodes the others (PNG stand-in,
     progressive) on the host; the chunk message carries both kinds and splits back into the same packs."""
     from irn_b200.step import _common
     from irn_b200.voc12 import dataloader
@@ -130,8 +131,8 @@ def test_loader_routes_bytes_and_host_pixels(tmp_path):
     assert _common.size_key(packs[0]) == _common.size_key({"size": packs[0]["size"], "img_u8": host["img_u8"][:, :24]})
     one = _common.collate_one([dict(items[0])])
     assert "jpeg_exact" in one and one["size"] == (24, 40)
-    # the raw-image steps (cam_to_ir_label) ship bytes too; nvJPEG keeps its own key
+    # the raw-image steps (cam_to_ir_label) ship bytes too; --device_jpeg True is the exact decoder
     raw = _common.make_dataset(args, str(root / "list.txt"), (1.0,), raw_images=True)
     assert "jpeg_exact" in raw[0]
-    nv = _common.make_dataset(types.SimpleNamespace(**dict(vars(args), device_jpeg=True)), str(root / "list.txt"), (1.0,))
-    assert "jpeg" in nv[0] and "jpeg_exact" not in nv[0]
+    on = _common.make_dataset(types.SimpleNamespace(**dict(vars(args), device_jpeg=True)), str(root / "list.txt"), (1.0,))
+    assert "jpeg_exact" in on[0] and "img_u8" not in on[0]

@@ -1,7 +1,7 @@
 """JPEG decode timing on batches of seeded synthetic 375x500 / 500x375 files (4:2:0, quality 90, half of each orientation): the exact
-device decoder (irn_b200.jpeg.ExactJpegDecoder) split into its four stages with CUDA events, nvJPEG (irn_b200.jpeg.JpegDecoder, one
-call per image size) and PIL on a pool of host threads, all on the same files; then make_cam and make_sem_seg_labels over a
-mixed-size synthetic JPEG list with the host decoder and with --device_jpeg exact, run alternately.  Medians after warm-up.
+device decoder (irn_b200.jpeg.ExactJpegDecoder) split into its four stages with CUDA events and PIL on a pool of host threads, both
+on the same files; then make_cam and make_sem_seg_labels over a mixed-size synthetic JPEG list with the host decoder and with
+--device_jpeg True, run alternately.  Medians after warm-up.
 
     python tools/jpeg_micro.py [--batch 32] [--reps 3] [--step_images 128] [--out results.json]
 """
@@ -64,7 +64,7 @@ def decoders(batch, reps):
     import torch
     from PIL import Image
     from irn_b200 import _lib
-    from irn_b200.jpeg import ExactJpegDecoder, JpegDecoder
+    from irn_b200.jpeg import ExactJpegDecoder
     streams = files(batch)
     dev = torch.device("cuda:0")
     exact = ExactJpegDecoder(dev)
@@ -83,17 +83,6 @@ def decoders(batch, reps):
     d, h = timed(lambda: exact.decode_packed(streams, check=False), reps)
     rows["exact_ms_per_batch"] = {"device": d, "host_wall": h, "unstuff": float(med[0]), "entropy": float(med[1]), "idct": float(med[2]),
                                   "upsample_colour": float(med[3])}
-    nv = JpegDecoder(dev)
-    groups = [[s for i, s in enumerate(streams) if i % 2 == k] for k in range(2)]
-    sizes = [(375, 500), (500, 375)]
-
-    def run_nv():
-        for g, s in zip(groups, sizes):
-            nv.decode(g, size=s)
-    for _ in range(3):
-        run_nv()
-    d, h = timed(run_nv, reps)
-    rows["nvjpeg_ms_per_batch"] = {"device": d, "host_wall": h, "backend": nv.backend, "calls": 2}
     with ThreadPoolExecutor(8) as pool:
         def pil():
             list(pool.map(lambda s: np.asarray(Image.open(io.BytesIO(s)).convert("RGB")), streams))
@@ -108,7 +97,7 @@ def decoders(batch, reps):
 
 
 def steps(n_images, rounds, workers):
-    """make_cam then make_sem_seg_labels over a mixed-size JPEG list, host decode vs --device_jpeg exact, alternately."""
+    """make_cam then make_sem_seg_labels over a mixed-size JPEG list, host decode vs --device_jpeg True, alternately."""
     import torch
     from irn_b200 import synth
     from irn_b200.step import make_cam, make_sem_seg_labels
