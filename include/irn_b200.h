@@ -122,7 +122,7 @@ int irn_rw_last_step_ms(float* ms_per_step, int* n_steps);
  * divide by the global max, prepend a constant background plane, argmax (ties -> lowest
  * index), map through keys.
  *
- *  rw   fp32 [C,h,w] one image;  keys_host HOST int32 [C+1] (entry 0 = background id, C+1 <= 64;
+ *  rw   fp32 [C,h,w] one image;  keys_host HOST int32 [C+1] (entry 0 = background id, C+1 <= 129;
  *  passed to the kernel by value: no copy, no synchronisation) or NULL (identity);  outputs, each optional (NULL): labels uint8 [H,W] = keys[argmax];
  *  index_out int32 [H,W] = raw argmax (instance path: C may exceed 255);  up_norm fp32
  *  [C,H,W] = normalised upsampled scores (instance scoring).  scratch: device, >= 16 bytes.
@@ -140,13 +140,16 @@ int irn_rw_labels(const float* rw, int C, int h, int w, int H, int W, float bg_t
  * blob holding the reference checkpoint's tensors in execution order (irn_b200/_pack.py):
  *   trunk: conv1.weight, bn1.{weight,bias,running_mean,running_var}; then per bottleneck
  *          conv1,bn1,conv2,bn2,conv3,bn3[,downsample.0,downsample.1] (weights OIHW);
- *   CAM  : + classifier.weight [20,2048];
+ *   CAM  : + classifier.weight [C,2048], C the number of classes: 20 (PASCAL VOC) for irn_cam_net_create, n_classes
+ *          (1..IRN_CAM_MAX_CLASSES; MS COCO has 80) for irn_cam_net_create_classes.  A C-class plan's CAMs are [.,C,.,.].
  *   IRN  : + fc_edge1..5 {conv.weight, gn.weight, gn.bias}, fc_edge6.{weight,bias},
  *          fc_dp1..7 {conv.weight, gn.weight, gn.bias}, fc_dp7.3.weight, mean_shift.running_mean.
  * FixedBatchNorm (eps 1e-5, inference statistics) is folded into the conv at creation.
  */
 typedef struct irn_net irn_net;
+#define IRN_CAM_MAX_CLASSES 128
 int irn_cam_net_create(const float* params, size_t n_floats, irn_net** out);
+int irn_cam_net_create_classes(const float* params, size_t n_floats, int n_classes, irn_net** out);
 int irn_irn_net_create(const float* params, size_t n_floats, irn_net** out);
 void irn_net_destroy(irn_net* net);
 /* Convolution arithmetic: 2 (default) = wgmma tensor cores, f16x3 split (fp16 hi/lo operand parts, per-k-block fp32 partial
@@ -163,13 +166,14 @@ int irn_net_get_conv_mode(const irn_net* net);
  *                       IRN_TAP_POOL  max pool output
  *                       IRN_TAP_BLOCK0 + 3 j + {0, 1, 2}: bottleneck j = 0..15 (layer1.0 .. layer4.2): t1 = relu(bn1(conv1)),
  *                       t2 = relu(bn2(conv2)), the block output
- *   CAM                 IRN_TAP_CAM_CLS  relu(classifier) [B,h,w,64] (channels 20..63 zero) in the tensor-core modes 1 and 2;
- *                       never written in mode 0, whose head kernel keeps it in registers
+ *   CAM                 IRN_TAP_CAM_CLS  relu(classifier) [B,h,w,64] (C <= 64) or [B,h,w,128] (channels C.. zero) in the
+ *                       tensor-core modes 1 and 2; never written in mode 0, whose head kernel keeps it in registers
  *   IRN                 IRN_TAP_HEAD0 + i: head i's raw 1x1 conv output (i = 0..4 fc_edge1..5, 5..11 fc_dp1..7);
  *                       IRN_TAP_ECAT the 160-channel edge concat, IRN_TAP_DCAT3 dp3|dp4|dp5, IRN_TAP_DCAT2 dp1|dp2|dp6,
  *                       IRN_TAP_DP7A relu(gn(fc_dp7 conv)), IRN_TAP_ELOG the edge logits [B,h,w,1], IRN_TAP_DLOG dp [B,h,w,2]
  * irn_net_tap_shape (host only) gives tap `id`'s NHWC shape for a forward of B samples: kind 0 (CAM) on an H x W input, kind 1
- * (IRN) on the crop_size x crop_size canvas (H, W unused); it fails for an id the kind does not have. */
+ * (IRN) on the crop_size x crop_size canvas (H, W unused); it fails for an id the kind does not have.  Kind 0 is a 20-class
+ * CAM plan; irn_cam_tap_shape gives the shapes of an n_classes CAM plan. */
 enum {
     IRN_TAP_STEM = 0,
     IRN_TAP_POOL = 1,
@@ -186,6 +190,7 @@ enum {
 };
 int irn_net_set_tap(irn_net* net, int id, float* dst, size_t bytes);
 int irn_net_tap_shape(int kind, int id, int B, int H, int W, int crop_size, int shape[4]);
+int irn_cam_tap_shape(int n_classes, int id, int B, int H, int W, int shape[4]);
 
 /* One convolution (+ folded FixedBatchNorm, residual add, ReLU) as a plan of its own: the building block of
  * the two networks above (net/resnet50.py:34-54), exposed for unit tests and for wiring other topologies.
@@ -220,18 +225,20 @@ int irn_shortcut_conv_forward(irn_conv* conv, const float* t2, const float* x, i
                               irn_stream_t stream);
 
 /* CAM.forward over B/2 (image, horizontally flipped image) pairs.
- *   x_nchw fp32 [B,3,H,W] (device), B even -> cam fp32 [B/2,20,ceil(H/16),ceil(W/16)]:
- *   relu(classifier(trunk(x)))[2p] + relu(...)[2p+1].flip(-1)   (net/resnet50_cam.py:65-68) */
+ *   x_nchw fp32 [B,3,H,W] (device), B even -> cam fp32 [B/2,C,ceil(H/16),ceil(W/16)], C the plan's classes:
+ *   relu(classifier(trunk(x)))[2p] + relu(...)[2p+1].flip(-1)   (net/resnet50_cam.py:65-68)
+ *   workspace: irn_cam_workspace_bytes for a 20-class plan, irn_cam_workspace_bytes_classes for any. */
 size_t irn_cam_workspace_bytes(int B, int H, int W);
+size_t irn_cam_workspace_bytes_classes(int B, int H, int W, int n_classes);
 int irn_cam_forward(const irn_net* net, const float* x_nchw, int B, int H, int W, float* cam_out,
                     void* workspace, size_t workspace_bytes, irn_stream_t stream);
 
 /* CAM.forward over B/2 pairs of different sizes on one canvas (irn_resize_ragged_forward lays it out).
  *   x_canvas fp32 [B,3,Hc,Wc] (device), B even: pair p (samples 2p, 2p+1) holds an image of hw[p] = (h_p, w_p) pixels at the
  *   top-left corner and +0.0 elsewhere; hw HOST int32 [B/2][2], 0 < h_p <= Hc, 0 < w_p <= Wc.
- *   -> cam fp32 [B/2,20,ceil(Hc/16),ceil(Wc/16)]: pair p's ceil(h_p/16) x ceil(w_p/16) corner is, bit for bit, what irn_cam_forward
+ *   -> cam fp32 [B/2,C,ceil(Hc/16),ceil(Wc/16)]: pair p's ceil(h_p/16) x ceil(w_p/16) corner is, bit for bit, what irn_cam_forward
  *   returns for that pair alone (the layers that read beyond an image's extent see zeros there, as they see padding alone); 0
- *   elsewhere.  workspace device, 256-byte aligned, >= irn_cam_workspace_bytes(B, Hc, Wc). */
+ *   elsewhere.  workspace device, 256-byte aligned, >= irn_cam_workspace_bytes_classes(B, Hc, Wc, C). */
 int irn_cam_forward_ragged(const irn_net* net, const float* x_canvas, int B, int Hc, int Wc, const int32_t* hw,
                            float* cam_out, void* workspace, size_t workspace_bytes, irn_stream_t stream);
 
@@ -260,14 +267,18 @@ int irn_edge_displacement_forward_ragged(const irn_net* net, const uint8_t* img_
 
 /* ------------------------------------------------------------------------------------
  * C4  multi-scale CAM merge.  Replaces step/make_cam.py:38-52.
- *   cams: HOST array of n_scales DEVICE pointers, each fp32 [20,hs[s],ws[s]] (CAM.forward outputs);
- *   (H,W) original image size; keys_host HOST int32 [K] = classes present (torch.nonzero(label)), by value;
+ *   cams: HOST array of n_scales DEVICE pointers, each fp32 [C,hs[s],ws[s]] (CAM.forward outputs), C = 20 for
+ *   irn_cam_merge, n_classes (1..IRN_CAM_MAX_CLASSES) for irn_cam_merge_classes;
+ *   (H,W) original image size; keys_host HOST int32 [K] = classes present (torch.nonzero(label)), K <= C, ids in [0, C);
  *   strided_out fp32 [K,ceil(H/4),ceil(W/4)], highres_out fp32 [K,H,W] (either may be NULL):
  *   sum over scales of the bilinear (align_corners=False) resample, each kept class / (max + 1e-5).
  *   scratch: device, >= 2*K*4 bytes. */
 int irn_cam_merge(const float* const* cams, const int* hs, const int* ws, int n_scales, int H, int W,
                   const int32_t* keys_host, int K, float* strided_out, float* highres_out,
                   void* scratch, irn_stream_t stream);
+int irn_cam_merge_classes(const float* const* cams, const int* hs, const int* ws, int n_scales, int n_classes, int H,
+                          int W, const int32_t* keys_host, int K, float* strided_out, float* highres_out,
+                          void* scratch, irn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------
  * P1-P4  instance path.  Replaces step/make_ins_seg_labels.py:18-105.

@@ -34,12 +34,14 @@ SIGNATURES = {
     "irn_rw_set_timing": (c_int, [c_int]),
     "irn_rw_last_step_ms": (c_int, [ctypes.POINTER(c_float), _p_int]),
     "irn_cam_net_create": (c_int, [c_void_p, c_size_t, ctypes.POINTER(c_void_p)]),
+    "irn_cam_net_create_classes": (c_int, [c_void_p, c_size_t, c_int, ctypes.POINTER(c_void_p)]),
     "irn_irn_net_create": (c_int, [c_void_p, c_size_t, ctypes.POINTER(c_void_p)]),
     "irn_net_destroy": (None, [c_void_p]),
     "irn_net_set_conv_mode": (c_int, [c_void_p, c_int]),
     "irn_net_get_conv_mode": (c_int, [c_void_p]),
     "irn_net_set_tap": (c_int, [c_void_p, c_int, c_void_p, c_size_t]),
     "irn_net_tap_shape": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _p_int]),
+    "irn_cam_tap_shape": (c_int, [c_int, c_int, c_int, c_int, c_int, _p_int]),
     "irn_conv_create": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
     "irn_conv_destroy": (None, [c_void_p]),
     "irn_conv_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p]),
@@ -50,6 +52,7 @@ SIGNATURES = {
     "irn_shortcut_conv_create": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, ctypes.POINTER(c_void_p)]),
     "irn_shortcut_conv_forward": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
     "irn_cam_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "irn_cam_workspace_bytes_classes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "irn_cam_forward": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "irn_cam_forward_ragged": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "irn_edge_displacement_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
@@ -60,6 +63,8 @@ SIGNATURES = {
                                                      c_void_p, c_void_p, c_size_t, c_void_p]),
     "irn_cam_merge": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                               c_void_p]),
+    "irn_cam_merge_classes": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                      c_void_p, c_void_p]),
     "irn_find_centroids": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "irn_connected_components": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "irn_cluster_scratch_bytes": (c_size_t, [c_int, c_int]),

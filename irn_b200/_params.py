@@ -45,17 +45,23 @@ class _Trunk(nn.Module):
             setattr(self, "layer%d" % i, nn.Sequential(*seq))
 
 
-class CamParams(nn.Module):
-    """Key-compatible with net/resnet50_cam.py:9-23 (Net / CAM)."""
+MAX_CLASSES = 128   # IRN_CAM_MAX_CLASSES of include/irn_b200.h
 
-    def __init__(self):
+
+class CamParams(nn.Module):
+    """Key-compatible with net/resnet50_cam.py:9-23 (Net / CAM).  The classifier has `n_classes` rows: 20 for PASCAL VOC (the
+    reference), 80 for MS COCO."""
+
+    def __init__(self, n_classes=20):
         super().__init__()
+        if not 1 <= int(n_classes) <= MAX_CLASSES:
+            raise ValueError("a CAM network has 1..%d classes, got %s" % (MAX_CLASSES, n_classes))
         t = self.resnet50 = _Trunk()
         self.stage1 = nn.Sequential(t.conv1, t.bn1, t.relu, t.maxpool, t.layer1)
         self.stage2 = nn.Sequential(t.layer2)
         self.stage3 = nn.Sequential(t.layer3)
         self.stage4 = nn.Sequential(t.layer4)
-        self.classifier = _conv(2048, 20, 1)
+        self.classifier = _conv(2048, int(n_classes), 1)
         self.backbone = nn.ModuleList([self.stage1, self.stage2, self.stage3, self.stage4])
         self.newly_added = nn.ModuleList([self.classifier])
 

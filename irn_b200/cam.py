@@ -12,7 +12,7 @@ import numpy as np
 import torch
 
 from . import _lib, _pack
-from ._params import CamParams
+from ._params import MAX_CLASSES, CamParams
 from .indexing import _workspace
 
 
@@ -39,16 +39,24 @@ class _Plan:
                    "irn_net_set_tap")
 
 
-def tap_shape(kind, tap_id, B, H=0, W=0, crop_size=0):
-    """NHWC shape of tap `tap_id` (irn_net_tap_shape) for a forward of B samples: kind 0 = CAM on H x W, 1 = IRNet on crop_size."""
+def tap_shape(kind, tap_id, B, H=0, W=0, crop_size=0, n_classes=20):
+    """NHWC shape of tap `tap_id` (irn_net_tap_shape) for a forward of B samples: kind 0 = CAM of `n_classes` classes on H x W,
+    1 = IRNet on crop_size."""
     shape = (ctypes.c_int * 4)()
-    _lib.check(_lib.lib().irn_net_tap_shape(int(kind), int(tap_id), int(B), int(H), int(W), int(crop_size), shape), "irn_net_tap_shape")
+    if kind == 0 and n_classes != 20:
+        _lib.check(_lib.lib().irn_cam_tap_shape(int(n_classes), int(tap_id), int(B), int(H), int(W), shape), "irn_cam_tap_shape")
+    else:
+        _lib.check(_lib.lib().irn_net_tap_shape(int(kind), int(tap_id), int(B), int(H), int(W), int(crop_size), shape),
+                   "irn_net_tap_shape")
     return tuple(shape)
 
 
 class CAM(CamParams):
-    def __init__(self):
-        super().__init__()
+    """The class count C follows the checkpoint: load_state_dict takes it from `classifier.weight` ([C,2048,1,1], 1 <= C <= 128;
+    20 for PASCAL VOC, 80 for MS COCO), and every forward returns C CAM planes per image."""
+
+    def __init__(self, n_classes=20):
+        super().__init__(n_classes)
         self._plan = None
         self._conv_mode = None      # None = the library's default for this network
 
@@ -74,23 +82,35 @@ class CAM(CamParams):
     def _invalidate(self):
         self._plan = None
 
-    def load_state_dict(self, *a, **k):
+    @property
+    def n_classes(self):
+        return int(self.classifier.weight.shape[0])
+
+    def load_state_dict(self, state_dict, *a, **k):
         self._invalidate()
-        return super().load_state_dict(*a, **k)
+        w = state_dict.get("classifier.weight") if hasattr(state_dict, "get") else None
+        if w is not None and tuple(w.shape[1:]) == (2048, 1, 1) and int(w.shape[0]) != self.n_classes:
+            C = int(w.shape[0])
+            if not 1 <= C <= MAX_CLASSES:
+                raise _lib.IrnError("CAM checkpoint has a %d-class classifier; 1..%d classes are supported" % (C, MAX_CLASSES))
+            self.classifier = torch.nn.Conv2d(2048, C, 1, bias=False)
+            self.newly_added = torch.nn.ModuleList([self.classifier])
+        return super().load_state_dict(state_dict, *a, **k)
 
     def _get_plan(self, device):
         if self._plan is None or self._plan.device != device:
             blob = _pack.pack_cam(self.state_dict())
             h = ctypes.c_void_p()
             with torch.cuda.device(device):
-                _lib.check(_lib.lib().irn_cam_net_create(blob.ctypes.data, blob.size, ctypes.byref(h)), "irn_cam_net_create")
+                _lib.check(_lib.lib().irn_cam_net_create_classes(blob.ctypes.data, blob.size, self.n_classes, ctypes.byref(h)),
+                           "irn_cam_net_create")
             self._plan = _Plan(h, device)
             if self._conv_mode is not None:
                 _lib.check(_lib.lib().irn_net_set_conv_mode(h, self._conv_mode), "irn_net_set_conv_mode")
         return self._plan
 
     def forward_batch(self, x):
-        """x cuda fp32 [2P,3,H,W] (P image/flip pairs of equal size) -> [P,20,ceil(H/16),ceil(W/16)]."""
+        """x cuda fp32 [2P,3,H,W] (P image/flip pairs of equal size) -> [P,C,ceil(H/16),ceil(W/16)]."""
         _lib.require_cuda(x)
         if x.dim() != 4 or x.shape[1] != 3 or x.shape[0] % 2:
             raise _lib.IrnError("CAM expects [2P,3,H,W] (image, flipped image) pairs, got %s" % (tuple(x.shape),))
@@ -99,8 +119,8 @@ class CAM(CamParams):
         L = _lib.lib()
         plan = self._get_plan(x.device)
         h, w = (H - 1) // 16 + 1, (W - 1) // 16 + 1
-        out = torch.empty((B // 2, 20, h, w), dtype=torch.float32, device=x.device)
-        need = L.irn_cam_workspace_bytes(B, H, W)
+        out = torch.empty((B // 2, self.n_classes, h, w), dtype=torch.float32, device=x.device)
+        need = L.irn_cam_workspace_bytes_classes(B, H, W, self.n_classes)
         ws = _workspace(need, x.device)
         with torch.cuda.device(x.device):
             rc = L.irn_cam_forward(plan.handle, _lib.ptr(x), B, H, W, _lib.ptr(out), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
@@ -109,7 +129,7 @@ class CAM(CamParams):
 
     def forward_ragged(self, canvas, extents):
         """Pairs of different sizes in one forward: canvas cuda fp32 [2P,3,Hc,Wc] with pair i's image and its flip of extents[i] =
-        (h_i, w_i) pixels at the top-left corner and +0.0 elsewhere (preprocess.resize_normalize_ragged) -> [P,20,ceil(Hc/16),ceil(Wc/16)]:
+        (h_i, w_i) pixels at the top-left corner and +0.0 elsewhere (preprocess.resize_normalize_ragged) -> [P,C,ceil(Hc/16),ceil(Wc/16)]:
         pair i's ceil(h_i/16) x ceil(w_i/16) corner equals, bit for bit, forward_batch of that pair alone; the rest is 0."""
         _lib.require_cuda(canvas)
         if canvas.dim() != 4 or canvas.shape[1] != 3 or canvas.shape[0] % 2 or canvas.dtype != torch.float32:
@@ -122,8 +142,8 @@ class CAM(CamParams):
             raise _lib.IrnError("CAM.forward_ragged: %d extents for %d pairs" % (hw.shape[0], B // 2))
         L = _lib.lib()
         plan = self._get_plan(x.device)
-        out = torch.empty((B // 2, 20, (H - 1) // 16 + 1, (W - 1) // 16 + 1), dtype=torch.float32, device=x.device)
-        ws = _workspace(L.irn_cam_workspace_bytes(B, H, W), x.device)
+        out = torch.empty((B // 2, self.n_classes, (H - 1) // 16 + 1, (W - 1) // 16 + 1), dtype=torch.float32, device=x.device)
+        ws = _workspace(L.irn_cam_workspace_bytes_classes(B, H, W, self.n_classes), x.device)
         with torch.cuda.device(x.device):
             rc = L.irn_cam_forward_ragged(plan.handle, _lib.ptr(x), B, H, W, hw.ctypes.data, _lib.ptr(out), _lib.ptr(ws), ws.numel(),
                                           _lib.stream_ptr())
@@ -131,7 +151,7 @@ class CAM(CamParams):
         return out
 
     def forward(self, x):
-        """Reference signature (net/resnet50_cam.py:55-70): [2,3,h,w] -> [20,ceil(h/16),ceil(w/16)]."""
+        """Reference signature (net/resnet50_cam.py:55-70): [2,3,h,w] -> [C,ceil(h/16),ceil(w/16)]."""
         return self.forward_batch(x)[0]
 
 

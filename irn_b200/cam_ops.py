@@ -5,21 +5,22 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._params import MAX_CLASSES
 
 
 _scratches = {}
 
 
 def _scratch(dev):
-    """2 x 20 per-class maxima (int-ordered float bits); one persistent buffer per device, reused in stream order."""
+    """2 x K <= 2 x 128 per-class maxima (int-ordered float bits); one persistent buffer per device, reused in stream order."""
     key = dev.index
     if key not in _scratches:
-        _scratches[key] = torch.empty(64, dtype=torch.int32, device=dev)
+        _scratches[key] = torch.empty(2 * MAX_CLASSES, dtype=torch.int32, device=dev)
     return _scratches[key]
 
 
 def merge_cams(outputs, size, label, want_highres=True):
-    """outputs: list of cuda fp32 [20,h_s,w_s] (one per scale); size=(H,W); label: fp32[20] multi-hot (any device).
+    """outputs: list of cuda fp32 [C,h_s,w_s] (one per scale); size=(H,W); label: fp32[C] multi-hot (any device).
     Returns (keys LongTensor[K] on cpu, strided_cam cuda [K,ceil(H/4),ceil(W/4)], highres_cam cuda [K,H,W] or None)."""
     L = _lib.lib()
     _lib.require_cuda(*outputs)
@@ -40,7 +41,7 @@ def merge_cams(outputs, size, label, want_highres=True):
     keys_host = np.ascontiguousarray(keys.numpy().astype(np.int32))
     scratch = _scratch(dev)
     with torch.cuda.device(dev):
-        rc = L.irn_cam_merge(ptrs, hs, ws, n, H, W, keys_host.ctypes.data, K, _lib.ptr(strided), _lib.ptr(highres), _lib.ptr(scratch),
-                             _lib.stream_ptr())
+        rc = L.irn_cam_merge_classes(ptrs, hs, ws, n, int(outs[0].shape[0]), H, W, keys_host.ctypes.data, K, _lib.ptr(strided),
+                                     _lib.ptr(highres), _lib.ptr(scratch), _lib.stream_ptr())
     _lib.check(rc, "irn_cam_merge")
     return keys, strided, highres

@@ -62,10 +62,12 @@ def dense_crf(images_u8, labels, n_labels, t=10, gt_prob=0.7, gauss=(3.0, 3.0), 
     return out, q, counts
 
 
-def ir_labels(images_u8, high_res_list, keys_list, fg, bg, return_counts=False, max_workspace_bytes=MAX_WORKSPACE_BYTES):
+def ir_labels(images_u8, high_res_list, keys_list, fg, bg, return_counts=False, max_workspace_bytes=MAX_WORKSPACE_BYTES, n_classes=20):
     """step/cam_to_ir_label.py:19-41 for a batch of equally-sized images: images_u8 uint8 [n,H,W,3] (CUDA), high_res_list[i] fp32
     [K_i,H,W] (make_cam's `high_res`; host or device), keys_list[i] int [K_i] (make_cam's `keys`), fg / bg = conf_fg_thres /
-    conf_bg_thres -> uint8 [n,H,W] conf maps (0 = background, 255 = unsure, else class + 1) on the images' device."""
+    conf_bg_thres -> uint8 [n,H,W] conf maps (0 = background, 255 = unsure, else class + 1) on the images' device.
+    n_classes: the dataset's class count (20 PASCAL VOC, 80 MS COCO; at most max_labels() - 1): every key must be a class id in
+    [0, n_classes), so an image has at most n_classes classes."""
     images_u8 = _check_images(images_u8)
     n, H, W = images_u8.shape[:3]
     if len(high_res_list) != n or len(keys_list) != n:
@@ -77,8 +79,14 @@ def ir_labels(images_u8, high_res_list, keys_list, fg, bg, return_counts=False, 
     for i, h in enumerate(high_res_list):
         if tuple(h.shape) != (counts[i], H, W):
             raise _lib.IrnError("ir_labels: high_res %d has shape %s, want %s" % (i, tuple(h.shape), (int(counts[i]), H, W)))
-    if counts.max(initial=0) + 1 > max_labels():
-        raise _lib.IrnError("ir_labels: %d classes in one image (at most %d)" % (counts.max(), max_labels() - 1))
+    if not 1 <= int(n_classes) <= max_labels() - 1:
+        raise _lib.IrnError("ir_labels: n_classes=%s outside [1, %d]" % (n_classes, max_labels() - 1))
+    if counts.max(initial=0) > n_classes:
+        raise _lib.IrnError("ir_labels: %d classes in one image (the dataset has %d)" % (counts.max(), n_classes))
+    for i, k in enumerate(keys):
+        if k.size and (k.min() < 0 or k.max() >= n_classes):
+            raise _lib.IrnError("ir_labels: image %d has class id %d outside [0, %d)" % (i, k.max() if k.max() >= n_classes else k.min(),
+                                                                                        n_classes))
     planes = [torch.as_tensor(h, dtype=torch.float32) for h in high_res_list if h.shape[0] > 0]
     high = torch.cat([p.to(dev) for p in planes], 0).contiguous() if planes else None
     keys_all = np.ascontiguousarray(np.concatenate(keys + [np.zeros(0, np.int64)]).astype(np.int32))

@@ -9,10 +9,10 @@ namespace irn {
 constexpr int kMaxScales = 8;
 
 struct MergeArgs {
-    const float* cam[kMaxScales];   // each [20, hs, ws]
+    const float* cam[kMaxScales];   // each [C, hs, ws]
     int hs[kMaxScales], ws[kMaxScales];
     int n_scales, n_cls;
-    int keys[20];                   // classes present (<= 20), by value
+    int keys[IRN_CAM_MAX_CLASSES];  // classes present (<= C), by value
 };
 
 __device__ __forceinline__ void src_index(int dst, float scale, int in_size, int& i0, int& i1, float& l1) {
@@ -64,20 +64,24 @@ __global__ void cam_norm_kernel(float* __restrict__ x, const int* __restrict__ m
 
 using namespace irn;
 
-extern "C" int irn_cam_merge(const float* const* cams, const int* hs, const int* ws, int n_scales, int H, int W, const int32_t* keys_host,
-                             int K, float* strided_out, float* highres_out, void* scratch, irn_stream_t stream_) {
+extern "C" int irn_cam_merge_classes(const float* const* cams, const int* hs, const int* ws, int n_scales, int n_classes, int H, int W,
+                                     const int32_t* keys_host, int K, float* strided_out, float* highres_out, void* scratch,
+                                     irn_stream_t stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     launch_counter() = 0;
     if (!cams || !hs || !ws || !scratch || n_scales <= 0 || n_scales > kMaxScales || H <= 0 || W <= 0 || K < 0)
         return fail(kBadArg, "irn_cam_merge: bad argument (n_scales must be 1..%d)", kMaxScales);
     if (K == 0) return kOk;
     if (!keys_host || (!strided_out && !highres_out)) return fail(kBadArg, "irn_cam_merge: null pointer");
-    if (K > 20) return fail(kBadArg, "irn_cam_merge: K=%d exceeds the 20 VOC classes", K);
+    if (n_classes < 1 || n_classes > IRN_CAM_MAX_CLASSES)
+        return fail(kBadArg, "irn_cam_merge: %d classes, need 1..%d", n_classes, IRN_CAM_MAX_CLASSES);
+    if (K > n_classes) return fail(kBadArg, "irn_cam_merge: K=%d exceeds the %d classes", K, n_classes);
     MergeArgs a;
     a.n_scales = n_scales;
-    a.n_cls = 20;
+    a.n_cls = n_classes;
     for (int k = 0; k < K; ++k) {
-        if (keys_host[k] < 0 || keys_host[k] >= 20) return fail(kBadArg, "irn_cam_merge: class id %d out of range", keys_host[k]);
+        if (keys_host[k] < 0 || keys_host[k] >= n_classes)
+            return fail(kBadArg, "irn_cam_merge: class id %d out of range [0, %d)", keys_host[k], n_classes);
         a.keys[k] = keys_host[k];
     }
     for (int s = 0; s < n_scales; ++s) {
@@ -104,4 +108,9 @@ extern "C" int irn_cam_merge(const float* const* cams, const int* hs, const int*
         IRN_LAUNCH_CHECK("cam_norm_kernel(highres)");
     }
     return kOk;
+}
+
+extern "C" int irn_cam_merge(const float* const* cams, const int* hs, const int* ws, int n_scales, int H, int W, const int32_t* keys_host,
+                             int K, float* strided_out, float* highres_out, void* scratch, irn_stream_t stream_) {
+    return irn_cam_merge_classes(cams, hs, ws, n_scales, 20, H, W, keys_host, K, strided_out, highres_out, scratch, stream_);
 }

@@ -234,10 +234,14 @@ __global__ void conv1x1_smalln_kernel(const float* __restrict__ x, const float* 
     }
 }
 
-// CAM head (net/resnet50_cam.py:65-68): relu(conv1x1 2048->20) of sample 2p at (y,x) plus the same of the
-// flipped sample 2p+1 at (y, w-1-x).  feat NHWC [2P,h,w,Cin] -> out NCHW-like [P,20,h,w].
+// The SIMT CAM heads take the classifier's rows kCamChunk at a time from a [ceil(C/kCamChunk)*kCamChunk][Cin] copy whose rows
+// C.. are zero: each class's dot product is the same sequence of operations whatever C is
+constexpr int kCamChunk = 20;
+
+// CAM head (net/resnet50_cam.py:65-68): relu(conv1x1 2048->C) of sample 2p at (y,x) plus the same of the
+// flipped sample 2p+1 at (y, w-1-x).  feat NHWC [2P,h,w,Cin] -> out NCHW-like [P,C,h,w].
 __global__ void cam_head_kernel(const float* __restrict__ feat, const float* __restrict__ w, float* __restrict__ out, int P, int h,
-                                int wd, int Cin) {
+                                int wd, int Cin, int C) {
     const size_t wid = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     const size_t n_pix = (size_t)P * h * wd;
@@ -245,26 +249,29 @@ __global__ void cam_head_kernel(const float* __restrict__ feat, const float* __r
     const int x = (int)(wid % wd);
     const int y = (int)((wid / wd) % h);
     const int p = (int)(wid / ((size_t)wd * h));
-    float a0[20], a1[20];
-    smalln_dot<20>(feat + ((((size_t)(2 * p) * h + y) * wd) + x) * Cin, w, Cin, lane, a0);
-    smalln_dot<20>(feat + ((((size_t)(2 * p + 1) * h + y) * wd) + (wd - 1 - x)) * Cin, w, Cin, lane, a1);
-    if (lane == 0) {
+    for (int n0 = 0; n0 < C; n0 += kCamChunk) {
+        float a0[kCamChunk], a1[kCamChunk];
+        smalln_dot<kCamChunk>(feat + ((((size_t)(2 * p) * h + y) * wd) + x) * Cin, w + (size_t)n0 * Cin, Cin, lane, a0);
+        smalln_dot<kCamChunk>(feat + ((((size_t)(2 * p + 1) * h + y) * wd) + (wd - 1 - x)) * Cin, w + (size_t)n0 * Cin, Cin, lane, a1);
+        if (lane == 0) {
 #pragma unroll
-        for (int n = 0; n < 20; ++n) out[(((size_t)p * 20 + n) * h + y) * wd + x] = fmaxf(a0[n], 0.f) + fmaxf(a1[n], 0.f);
+            for (int n = 0; n < kCamChunk; ++n)
+                if (n0 + n < C) out[(((size_t)p * C + n0 + n) * h + y) * wd + x] = fmaxf(a0[n], 0.f) + fmaxf(a1[n], 0.f);
+        }
     }
 }
 
-// CAM head tail for the tensor-core path: y = relu(classifier(x)) is already in t NHWC [2P,h,w,C] (first 20 channels real);
+// CAM head tail for the tensor-core path: y = relu(classifier(x)) is already in t NHWC [2P,h,w,Ct] (first C channels real);
 // out[p,n,y,x] = t[2p,y,x,n] + t[2p+1,y,w-1-x,n]      (net/resnet50_cam.py:68)
-__global__ void cam_flip_add_kernel(const float* __restrict__ t, float* __restrict__ out, int P, int h, int w, int C) {
+__global__ void cam_flip_add_kernel(const float* __restrict__ t, float* __restrict__ out, int P, int h, int w, int Ct, int C) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (size_t)P * 20 * h * w) return;
+    if (i >= (size_t)P * C * h * w) return;
     const int x = (int)(i % w);
     const int y = (int)((i / w) % h);
-    const int n = (int)((i / ((size_t)w * h)) % 20);
-    const int p = (int)(i / ((size_t)w * h * 20));
-    const float a = t[(((size_t)(2 * p) * h + y) * w + x) * C + n];
-    const float b = t[(((size_t)(2 * p + 1) * h + y) * w + (w - 1 - x)) * C + n];
+    const int n = (int)((i / ((size_t)w * h)) % C);
+    const int p = (int)(i / ((size_t)w * h * C));
+    const float a = t[(((size_t)(2 * p) * h + y) * w + x) * Ct + n];
+    const float b = t[(((size_t)(2 * p + 1) * h + y) * w + (w - 1 - x)) * Ct + n];
     out[i] = a + b;
 }
 
@@ -482,39 +489,43 @@ __global__ void zero_outside_kernel(float* __restrict__ x, int H, int W, int C, 
 }
 
 // cam_flip_add_kernel for pair p = i0 + blockIdx.y of a ragged batch: inside its CAM extent he x we the flipped sample is read at
-// (y, we-1-x), i.e. flipped within the pair's own width; outside the extent the output is 0.  grid (ceil(20*h*w / 256), n)
-__global__ void cam_flip_add_ragged_kernel(const float* __restrict__ t, float* __restrict__ out, int h, int w, int C, PairExtents e, int i0) {
+// (y, we-1-x), i.e. flipped within the pair's own width; outside the extent the output is 0.  grid (ceil(C*h*w / 256), n)
+__global__ void cam_flip_add_ragged_kernel(const float* __restrict__ t, float* __restrict__ out, int h, int w, int Ct, int C, PairExtents e,
+                                           int i0) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= 20 * h * w) return;
+    if (i >= C * h * w) return;
     const int j = blockIdx.y, p = i0 + j;
     const int x = i % w, y = (i / w) % h, n = i / (w * h);
     const int we = e.w[j];
     float v = 0.f;
     if (y < e.h[j] && x < we)
-        v = t[(((size_t)(2 * p) * h + y) * w + x) * C + n] + t[(((size_t)(2 * p + 1) * h + y) * w + (we - 1 - x)) * C + n];
-    out[(size_t)p * 20 * h * w + i] = v;
+        v = t[(((size_t)(2 * p) * h + y) * w + x) * Ct + n] + t[(((size_t)(2 * p + 1) * h + y) * w + (we - 1 - x)) * Ct + n];
+    out[(size_t)p * C * h * w + i] = v;
 }
 
 // cam_head_kernel for pair p = i0 + blockIdx.y of a ragged batch, flipped within the pair's CAM width; 0 outside its extent.
 // grid (ceil(h*w*32 / 256), n)
 __global__ void cam_head_ragged_kernel(const float* __restrict__ feat, const float* __restrict__ w, float* __restrict__ out, int h, int wd,
-                                       int Cin, PairExtents e, int i0) {
+                                       int Cin, int C, PairExtents e, int i0) {
     const int wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (wid >= h * wd) return;
     const int j = blockIdx.y, p = i0 + j;
     const int x = wid % wd, y = wid / wd, we = e.w[j];
-    float* o = out + (size_t)p * 20 * h * wd + (size_t)y * wd + x;
+    float* o = out + (size_t)p * C * h * wd + (size_t)y * wd + x;
     if (y >= e.h[j] || x >= we) {
-        if (lane < 20) o[(size_t)lane * h * wd] = 0.f;
+        for (int n = lane; n < C; n += 32) o[(size_t)n * h * wd] = 0.f;
         return;
     }
-    float a0[20], a1[20];
-    smalln_dot<20>(feat + ((((size_t)(2 * p) * h + y) * wd) + x) * Cin, w, Cin, lane, a0);
-    smalln_dot<20>(feat + ((((size_t)(2 * p + 1) * h + y) * wd) + (we - 1 - x)) * Cin, w, Cin, lane, a1);
-    if (lane == 0) {
+    for (int n0 = 0; n0 < C; n0 += kCamChunk) {
+        float a0[kCamChunk], a1[kCamChunk];
+        smalln_dot<kCamChunk>(feat + ((((size_t)(2 * p) * h + y) * wd) + x) * Cin, w + (size_t)n0 * Cin, Cin, lane, a0);
+        smalln_dot<kCamChunk>(feat + ((((size_t)(2 * p + 1) * h + y) * wd) + (we - 1 - x)) * Cin, w + (size_t)n0 * Cin, Cin, lane, a1);
+        if (lane == 0) {
 #pragma unroll
-        for (int n = 0; n < 20; ++n) o[(size_t)n * h * wd] = fmaxf(a0[n], 0.f) + fmaxf(a1[n], 0.f);
+            for (int n = 0; n < kCamChunk; ++n)
+                if (n0 + n < C) o[(size_t)(n0 + n) * h * wd] = fmaxf(a0[n], 0.f) + fmaxf(a1[n], 0.f);
+        }
     }
 }
 

@@ -25,7 +25,7 @@
 namespace irn {
 namespace crf {
 
-constexpr int kMaxLabels = 32;   // per CRF; VOC needs 21
+constexpr int kMaxLabels = IRN_CAM_MAX_CLASSES + 1;   // per CRF: background + every class of a CAM plan (VOC 21, COCO 81)
 constexpr int kCB = 8;           // value channels per pass through the lattice
 
 struct ImgParam {

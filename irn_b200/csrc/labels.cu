@@ -6,9 +6,11 @@
 
 namespace irn {
 
+constexpr int kMaxKeys = IRN_CAM_MAX_CLASSES + 1;
+
 struct LabelKeys {     // class id per argmax index (entry 0 = background), passed by value: no device copy, no host sync
     int n;
-    int v[64];
+    int v[kMaxKeys];
 };
 
 // torch upsample_bilinear2d, align_corners=False, scale_factor=4: src = max(0,(dst+0.5)/4-0.5)
@@ -91,7 +93,9 @@ extern "C" int irn_rw_labels(const float* rw, int C, int h, int w, int H, int W,
     LabelKeys keys;
     keys.n = 0;
     if (keys_host) {
-        if (C + 1 > 64) return fail(kUnsupported, "irn_rw_labels: a key table of %d entries exceeds 64 (pass NULL and map the index map on the host)", C + 1);
+        if (C + 1 > kMaxKeys)
+            return fail(kUnsupported, "irn_rw_labels: a key table of %d entries exceeds %d (pass NULL and map the index map on the host)", C + 1,
+                        kMaxKeys);
         keys.n = C + 1;
         for (int i = 0; i <= C; ++i) keys.v[i] = keys_host[i];
     }

@@ -71,8 +71,9 @@ struct irn_net {
     irn::Conv stem;
     std::vector<irn::Block> blocks[4];
     // CAM
-    float* classifier = nullptr;   // [20][2048] (SIMT head kernel)
-    irn::Conv cls_conv;            // the same weights as a 2048 -> 64 1x1 conv (rows 20..63 zero) for the tensor-core path
+    int n_classes = 20;            // C, the classifier's rows
+    float* classifier = nullptr;   // [ceil(C/kCamChunk)*kCamChunk][2048], rows C.. zero (SIMT head kernel)
+    irn::Conv cls_conv;            // the same weights as a 2048 -> 64 (C <= 64) or 128 1x1 conv, rows C.. zero, for the tensor-core path
     // IRN
     irn::Head edge[5], dp[7];
     float* edge6_w = nullptr;      // [1][160]
@@ -647,6 +648,9 @@ static int run_trunk(const irn_net* net, const float* x_nchw, int B, int H, int 
     return kOk;
 }
 
+// Rows of the tensor-core classifier conv of a C-class plan: C padded to a whole 64- or 128-wide N tile
+static inline int cls_rows(int n_classes) { return n_classes <= 64 ? 64 : 128; }
+
 static size_t trunk_workspace_floats(int B, int H, int W, bool keep) {
     TrunkShapes s = trunk_shapes(B, H, W);
     size_t n = stem_halo_floats(B, H, W) + (size_t)B * s.H1 * s.W1 * 64 + (size_t)B * s.H2 * s.W2 * 64 + 5 * s.max_act;
@@ -792,7 +796,7 @@ extern "C" int irn_net_set_tap(irn_net* net, int id, float* dst, size_t bytes) {
     return kOk;
 }
 
-extern "C" int irn_net_tap_shape(int kind, int id, int B, int H, int W, int crop_size, int shape[4]) {
+static int tap_shape(int kind, int n_classes, int id, int B, int H, int W, int crop_size, int shape[4]) {
     if (!shape || !(kind == 0 || kind == 1) || B <= 0) return fail(kBadArg, "irn_net_tap_shape: bad argument");
     if (kind == 1) H = W = crop_size;
     if (H <= 0 || W <= 0) return fail(kBadArg, "irn_net_tap_shape: bad input size %d x %d", H, W);
@@ -811,7 +815,7 @@ extern "C" int irn_net_tap_shape(int kind, int id, int B, int H, int W, int crop
         w = in_grid ? (l ? s.Wl[l - 1] : s.W2) : s.Wl[l];
         c = which == 2 ? 4 * kPlanes[l] : kPlanes[l];
     } else if (kind == 0 && id == IRN_TAP_CAM_CLS) {
-        h = s.Hl[3]; w = s.Wl[3]; c = 64;
+        h = s.Hl[3]; w = s.Wl[3]; c = cls_rows(n_classes);
     } else if (kind == 1 && id >= IRN_TAP_HEAD0 && id < IRN_TAP_COUNT) {
         // grid of each head's conv (edge1..5, dp1..7) and its channels; then ecat, dcat3, dcat2, dp7a, elog, dlog
         static const int lvl[18] = {0, 1, 2, 3, 3, 0, 1, 2, 3, 3, 2, 1, 1, 2, 1, 1, 1, 1};   // 0 = x1 grid, 1..3 = Hl[0..2]
@@ -827,22 +831,42 @@ extern "C" int irn_net_tap_shape(int kind, int id, int B, int H, int W, int crop
     return kOk;
 }
 
+extern "C" int irn_net_tap_shape(int kind, int id, int B, int H, int W, int crop_size, int shape[4]) {
+    return tap_shape(kind, 20, id, B, H, W, crop_size, shape);
+}
+
+extern "C" int irn_cam_tap_shape(int n_classes, int id, int B, int H, int W, int shape[4]) {
+    if (n_classes < 1 || n_classes > IRN_CAM_MAX_CLASSES)
+        return fail(kBadArg, "irn_cam_tap_shape: %d classes, need 1..%d", n_classes, IRN_CAM_MAX_CLASSES);
+    return tap_shape(0, n_classes, id, B, H, W, 0, shape);
+}
+
 extern "C" void irn_net_destroy(irn_net* net) { delete net; }
 
-extern "C" int irn_cam_net_create(const float* params, size_t n_floats, irn_net** out) {
+extern "C" int irn_cam_net_create_classes(const float* params, size_t n_floats, int n_classes, irn_net** out) {
     if (!params || !out) return fail(kBadArg, "irn_cam_net_create: null pointer");
+    if (n_classes < 1 || n_classes > IRN_CAM_MAX_CLASSES)
+        return fail(kBadArg, "irn_cam_net_create: %d classes, need 1..%d", n_classes, IRN_CAM_MAX_CLASSES);
     irn_net* net = new irn_net();
     net->kind = 0;
+    net->n_classes = n_classes;
     Reader rd{params, n_floats};
     int rc = read_trunk(net, rd);
     if (!rc) {
-        const float* cw = rd.p;
-        rc = read_vec(net->mem, rd, (size_t)20 * 2048, &net->classifier);
+        const size_t nw = (size_t)n_classes * 2048;
+        const float* cw = rd.take(nw);
+        if (!rd.ok) rc = fail(kBadArg, "parameter blob too short (classifier of %d classes)", n_classes);
         if (!rc) {
-            std::vector<float> padded((size_t)64 * 2048, 0.f);
-            std::memcpy(padded.data(), cw, (size_t)20 * 2048 * sizeof(float));
+            std::vector<float> simt((size_t)(n_classes + kCamChunk - 1) / kCamChunk * kCamChunk * 2048, 0.f);
+            std::memcpy(simt.data(), cw, nw * sizeof(float));
+            rc = upload(net->mem, simt, &net->classifier);
+        }
+        if (!rc) {
+            const int rows = cls_rows(n_classes);
+            std::vector<float> padded((size_t)rows * 2048, 0.f);
+            std::memcpy(padded.data(), cw, nw * sizeof(float));
             Reader r2{padded.data(), padded.size()};
-            rc = read_conv(net->mem, r2, net->cls_conv, 2048, 64, 1, 1, 0, false);
+            rc = read_conv(net->mem, r2, net->cls_conv, 2048, rows, 1, 1, 0, false);
         }
     }
     if (!rc && rd.left != 0) rc = fail(kBadArg, "irn_cam_net_create: %zu unread floats in the parameter blob", rd.left);
@@ -852,6 +876,10 @@ extern "C" int irn_cam_net_create(const float* params, size_t n_floats, irn_net*
     }
     *out = net;
     return kOk;
+}
+
+extern "C" int irn_cam_net_create(const float* params, size_t n_floats, irn_net** out) {
+    return irn_cam_net_create_classes(params, n_floats, 20, out);
 }
 
 extern "C" int irn_irn_net_create(const float* params, size_t n_floats, irn_net** out) {
@@ -879,11 +907,13 @@ extern "C" int irn_irn_net_create(const float* params, size_t n_floats, irn_net*
     return kOk;
 }
 
-extern "C" size_t irn_cam_workspace_bytes(int B, int H, int W) {
-    if (B <= 0 || (B & 1) || H <= 0 || W <= 0) return 0;
+extern "C" size_t irn_cam_workspace_bytes_classes(int B, int H, int W, int n_classes) {
+    if (B <= 0 || (B & 1) || H <= 0 || W <= 0 || n_classes < 1 || n_classes > IRN_CAM_MAX_CLASSES) return 0;
     const TrunkShapes sh = trunk_shapes(B, H, W);
-    return (trunk_workspace_floats(B, H, W, false) + (size_t)B * sh.Hl[3] * sh.Wl[3] * 64 + 128) * sizeof(float);
+    return (trunk_workspace_floats(B, H, W, false) + (size_t)B * sh.Hl[3] * sh.Wl[3] * cls_rows(n_classes) + 128) * sizeof(float);
 }
+
+extern "C" size_t irn_cam_workspace_bytes(int B, int H, int W) { return irn_cam_workspace_bytes_classes(B, H, W, 20); }
 
 // The CAM heads of a ragged batch (ext HOST [P][2] input extents): kernel(e, i0, n) launches the head of pairs i0 .. i0+n-1 with
 // their extents on the CAM grid in e
@@ -902,7 +932,7 @@ static int ragged_heads(const int32_t* ext, int P, Launch kernel) {
     return kOk;
 }
 
-// CAM.forward for P = B/2 (image, flipped image) pairs of x NCHW fp32 [B,3,H,W] -> cam [P,20,ceil(H/16),ceil(W/16)].  With `ext`
+// CAM.forward for P = B/2 (image, flipped image) pairs of x NCHW fp32 [B,3,H,W] -> cam [P,C,ceil(H/16),ceil(W/16)].  With `ext`
 // (HOST [P][2]), pair p is an image of ext[p] pixels at the top-left corner of the canvas, zero elsewhere (run_trunk): each pair's
 // head flips within its own CAM width and writes 0 outside its CAM extent.
 static int run_cam(const irn_net* net, const float* x_nchw, int B, int H, int W, const int32_t* ext, float* cam_out, Arena& ar,
@@ -911,39 +941,40 @@ static int run_cam(const irn_net* net, const float* x_nchw, int B, int H, int W,
     TrunkShapes sh;
     int rc = run_trunk(net, x_nchw, B, H, W, H, W, ar, false, feats, sh, st, nullptr, ext);
     if (rc) return rc;
-    const int P = B / 2, h = sh.Hl[3], w = sh.Wl[3];
+    const int P = B / 2, h = sh.Hl[3], w = sh.Wl[3], C = net->n_classes;
     if (net->conv_mode >= 1 && net->cls_conv.tf32.ok) {
-        // classifier as a 2048 -> 64 tensor-core conv with fused ReLU (the one-warp-per-pixel head re-reads the 160 KB weight
-        // matrix per pixel), then flip-add + NHWC -> NCHW on the 20 real channels
-        float* tmp = ar.take((size_t)B * h * w * 64);
+        // classifier as a 2048 -> 64 (or 128) tensor-core conv with fused ReLU (the one-warp-per-pixel head re-reads the weight
+        // matrix per pixel), then flip-add + NHWC -> NCHW on the C real channels
+        const int Ct = net->cls_conv.cout;
+        float* tmp = ar.take((size_t)B * h * w * Ct);
         if (!ar.ok) return fail(kWorkspace, "irn_cam_forward: workspace too small");
         if ((rc = run_conv(net->conv_mode, net->cls_conv, feats[4], B, h, w, nullptr, tmp, true, st, nullptr, nullptr))) return rc;
-        if ((rc = tap(net, IRN_TAP_CAM_CLS, tmp, (size_t)B * h * w * 64, st))) return rc;
+        if ((rc = tap(net, IRN_TAP_CAM_CLS, tmp, (size_t)B * h * w * Ct, st))) return rc;
         if (ext)
             return ragged_heads(ext, P, [&](const PairExtents& e, int i0, int n) -> int {
-                cam_flip_add_ragged_kernel<<<dim3((unsigned)((20 * h * w + 255) / 256), n), 256, 0, st>>>(tmp, cam_out, h, w, 64, e, i0);
+                cam_flip_add_ragged_kernel<<<dim3((unsigned)((C * h * w + 255) / 256), n), 256, 0, st>>>(tmp, cam_out, h, w, Ct, C, e, i0);
                 IRN_LAUNCH_CHECK("cam_flip_add_ragged_kernel");
                 return kOk;
             });
-        const size_t total = (size_t)P * 20 * h * w;
-        cam_flip_add_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(tmp, cam_out, P, h, w, 64);
+        const size_t total = (size_t)P * C * h * w;
+        cam_flip_add_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(tmp, cam_out, P, h, w, Ct, C);
         IRN_LAUNCH_CHECK("cam_flip_add_kernel");
         return kOk;
     }
     if (ext)
         return ragged_heads(ext, P, [&](const PairExtents& e, int i0, int n) -> int {
             cam_head_ragged_kernel<<<dim3((unsigned)((h * w * 32 + 255) / 256), n), 256, 0, st>>>(feats[4], net->classifier, cam_out, h, w,
-                                                                                              2048, e, i0);
+                                                                                              2048, C, e, i0);
             IRN_LAUNCH_CHECK("cam_head_ragged_kernel");
             return kOk;
         });
     const size_t warps = (size_t)P * h * w;
-    cam_head_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(feats[4], net->classifier, cam_out, P, h, w, 2048);
+    cam_head_kernel<<<(unsigned)((warps * 32 + 255) / 256), 256, 0, st>>>(feats[4], net->classifier, cam_out, P, h, w, 2048, C);
     IRN_LAUNCH_CHECK("cam_head_kernel");
     return kOk;
 }
 
-// CAM.forward for P = B/2 (image, flipped image) pairs: x NCHW fp32 [B,3,H,W] -> cam [P,20,ceil(H/16),ceil(W/16)]
+// CAM.forward for P = B/2 (image, flipped image) pairs: x NCHW fp32 [B,3,H,W] -> cam [P,C,ceil(H/16),ceil(W/16)]
 extern "C" int irn_cam_forward(const irn_net* net, const float* x_nchw, int B, int H, int W, float* cam_out, void* workspace,
                                size_t workspace_bytes, irn_stream_t stream_) {
     launch_counter() = 0;
@@ -1133,7 +1164,7 @@ extern "C" int irn_cam_forward_ragged(const irn_net* net, const float* x_canvas,
     if (!is_device_ptr(x_canvas) || !is_device_ptr(cam_out) || !is_device_ptr(workspace))
         return fail(kBadArg, "%s: canvas, output and workspace must be device memory", fn);
     if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "%s: workspace must be 256-byte aligned", fn);
-    if (workspace_bytes < irn_cam_workspace_bytes(B, Hc, Wc)) return fail(kWorkspace, "%s: workspace too small", fn);
+    if (workspace_bytes < irn_cam_workspace_bytes_classes(B, Hc, Wc, net->n_classes)) return fail(kWorkspace, "%s: workspace too small", fn);
     Arena ar{(char*)workspace, workspace_bytes};
     return run_cam(net, x_canvas, B, Hc, Wc, hw, cam_out, ar, (cudaStream_t)stream_);
 }

@@ -105,6 +105,10 @@ class EdgeDisplacement(IrnParams):
         P = len(sizes)
         if P == 0:
             raise _lib.IrnError("EdgeDisplacement.forward_ragged: empty batch")
+        S = int(self.crop_size)
+        for i, (h, w) in enumerate(sizes):
+            if max(h, w) > S:
+                raise _lib.IrnError("EdgeDisplacement: image %d is %dx%d, larger than crop_size %d (--irn_crop_size)" % (i, h, w, S))
         if flat.dtype != torch.uint8 or flat.dim() != 1:
             raise _lib.IrnError("EdgeDisplacement.forward_ragged expects uint8 images, got %s %s" % (flat.dtype, tuple(flat.shape)))
         dev = torch.device("cuda", torch.cuda.current_device()) if not flat.is_cuda else flat.device
@@ -114,7 +118,6 @@ class EdgeDisplacement(IrnParams):
         np.cumsum(hw[:-1, 0].astype(np.int64) * hw[:-1, 1] * 3, out=offs[1:])
         L = _lib.lib()
         plan = self._get_plan(dev)
-        S = int(self.crop_size)
         fc = (S - 1) // 4 + 1
         edge = torch.empty((P, 1, fc, fc), dtype=torch.float32, device=dev)
         dp = torch.empty((P, 2, fc, fc), dtype=torch.float32, device=dev)

@@ -22,6 +22,8 @@ import torch
 from . import cam_ops, indexing, instance, preprocess
 from .voc12 import dataloader as voc_data
 
+KNEE_PIXELS = 512 * 512   # the sub-batches below are sized for images up to this many pixels (PASCAL VOC's) and shrink beyond
+
 
 def preprocess_batch(images_u8, scales=(1.0, 0.5, 1.5, 2.0), pin=True):
     """C1 on the host (voc12/dataloader.py:185-205): list of uint8 [H,W,3] of one size -> list over scales of
@@ -49,6 +51,16 @@ class PseudoLabelPipeline:
         self._staging = {}
 
     # ------------------------------------------------------------------ stages
+    def _cam_sub_batch(self, scale, size):
+        """Image pairs per CAM forward at `scale`: cam_sub at scale 2.0, more at smaller scales, fewer for images above 512 x 512
+        pixels (MS COCO's reach 640), so that a forward's activation arena holds about cam_sub 1024 x 1024 canvases at most."""
+        big = min(1.0, float(KNEE_PIXELS) / (int(size[0]) * int(size[1])))
+        return max(1, int(self.cam_sub * (2.0 / scale) ** 2 * big))
+
+    def _irn_sub_batch(self):
+        """Images per IRNet forward: 4 cam_sub on the 512 x 512 canvas, fewer on a larger one (--irn_crop_size 640 for MS COCO)."""
+        return max(1, int(self.cam_sub * 4 * min(1.0, float(KNEE_PIXELS) / int(self.irn.crop_size) ** 2)))
+
     def _upload_u8(self, images_u8, slot="u8"):
         x = images_u8
         if not x.is_cuda:
@@ -79,7 +91,7 @@ class PseudoLabelPipeline:
 
     def cam_stage(self, xs, labels, size, want_highres=True, scales=None, ready=None, order=None):
         """C2-C4: per-scale CAM forward in sub-batches of image pairs, then merge + normalise per image
-        (step/make_cam.py:35-52).  xs: list over scales of cuda [2N,3,h_s,w_s]; labels [N,20] multi-hot.
+        (step/make_cam.py:35-52).  xs: list over scales of cuda [2N,3,h_s,w_s]; labels [N,C] multi-hot.
         Returns (keys: list of int64 arrays, strided: list of cuda [K_i,h4,w4], highres: list of cuda [K_i,H,W] or None)."""
         scales = self.scales if scales is None else tuple(scales)
         main = torch.cuda.current_stream(self.device)
@@ -91,7 +103,7 @@ class PseudoLabelPipeline:
                 main.wait_event(ready[k])
             # sub-batch so that every forward sees about the same number of pixels (cam_sub images at scale 2.0):
             # small scales batch more images to keep all SMs busy, large scales bound the activation arena
-            sub = max(1, int(self.cam_sub * (2.0 / s) ** 2))
+            sub = self._cam_sub_batch(s, size)
             outs = [self.cam.forward_batch(x[2 * i:2 * min(i + sub, N)]) for i in range(0, N, sub)]
             cams[k] = outs[0] if len(outs) == 1 else torch.cat(outs, 0)
         keys, strided, highres = [], [], []
@@ -104,7 +116,7 @@ class PseudoLabelPipeline:
 
     def cam_ragged_stage(self, images_u8, sizes, labels, want_highres=True, scales=None):
         """C1-C4 for images of different sizes: images_u8 one flat cuda uint8 buffer holding uint8 [H_i,W_i,3] back to back, sizes
-        [(H_i, W_i)], labels [N,20].  Per scale, the sub-batches of cam_stage, each on a canvas as large as its largest image
+        [(H_i, W_i)], labels [N,C].  Per scale, the sub-batches of cam_stage, each on a canvas as large as its largest image
         (preprocess.resize_normalize_ragged, CAM.forward_ragged); then merge + normalise per image on its own corner of the CAMs.
         Returns what cam_stage returns, each image's entries bit for bit those cam_stage gives for it."""
         scales = self.scales if scales is None else tuple(scales)
@@ -113,7 +125,7 @@ class PseudoLabelPipeline:
         offs = np.concatenate([[0], np.cumsum([3 * h * w for h, w in sizes])])
         cams = [[] for _ in range(N)]
         for s in scales:
-            sub = max(1, int(self.cam_sub * (2.0 / s) ** 2))     # as cam_stage
+            sub = self._cam_sub_batch(s, max(sizes, key=lambda hw: hw[0] * hw[1]))     # as cam_stage
             for i in range(0, N, sub):
                 j = min(i + sub, N)
                 canvas, ext = preprocess.resize_normalize_ragged(images_u8[int(offs[i]):int(offs[j])], sizes[i:j], s)
@@ -131,7 +143,7 @@ class PseudoLabelPipeline:
     def irn_stage(self, x1):
         """I1/I2: x1 cuda fp32 [2N,3,H,W] (scale-1.0 pyramid) -> (edge [N,h,w], dp [N,2,h,w])."""
         N = x1.shape[0] // 2
-        irn_sub = self.cam_sub * 4
+        irn_sub = self._irn_sub_batch()
         edges, dps = [], []
         for i in range(0, N, irn_sub):
             e, d = self.irn.forward_batch(x1[2 * i:2 * min(i + irn_sub, N)])
@@ -142,7 +154,7 @@ class PseudoLabelPipeline:
     def irn_ragged_stage(self, images_u8, sizes):
         """I1/I2 for images of different sizes: images_u8 one flat cuda uint8 buffer holding uint8 [H_i,W_i,3] back to back, sizes
         [(H_i, W_i)] -> (edge [N,fc,fc], dp [N,2,fc,fc]) on the crop_size canvas (EdgeDisplacement.forward_ragged)."""
-        irn_sub = self.cam_sub * 4
+        irn_sub = self._irn_sub_batch()
         offs = np.concatenate([[0], np.cumsum([3 * h * w for h, w in sizes])])
         edges, dps = [], []
         for i in range(0, len(sizes), irn_sub):
@@ -265,7 +277,7 @@ class PseudoLabelPipeline:
     @torch.no_grad()
     def run(self, inputs, labels, size, want_highres=True):
         """inputs: list over scales of [2N,3,h_s,w_s] fp32 (cuda, or pinned host -> copied here);
-        labels: [N,20] multi-hot; size=(H,W).  Returns dict with 'labels' uint8 cuda [N,H,W], 'keys' list,
+        labels: [N,C] multi-hot; size=(H,W).  Returns dict with 'labels' uint8 cuda [N,H,W], 'keys' list,
         'cams' list of cuda [K_i,h4,w4] and 'high_res' list (or None)."""
         dev = self.device
         # host inputs: copy on a side stream, one event per scale, so the forward of scale k overlaps the H2D of scale k+1..

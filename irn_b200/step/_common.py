@@ -195,8 +195,24 @@ class Batcher:
             self._flush(key)
 
 
+def dataset_name(args):
+    """--dataset voc12 (default) or coco."""
+    name = str(getattr(args, "dataset", "voc12") or "voc12")
+    if name not in ("voc12", "coco"):
+        raise ValueError("--dataset must be voc12 or coco, got %r" % name)
+    return name
+
+
+def n_classes(args):
+    """The class count of the dataset the step runs on: 20 for PASCAL VOC (and the synthetic images), 80 for MS COCO."""
+    if dataset_name(args) == "coco":
+        from ..coco.dataloader import N_CAT
+        return N_CAT
+    return voc_data.N_CAT
+
+
 def make_dataset(args, list_path, scales, cam_dir=None, cam_field="cam", raw_images=False):
-    """VOC images from --voc12_root, or seeded synthetic ones with --synthetic N.  `cam_dir`: the label steps let the loader
+    """VOC images from --voc12_root, MS COCO images from --coco_root with --dataset coco, or seeded synthetic ones with --synthetic N.  `cam_dir`: the label steps let the loader
     workers read the stored CAM dicts (batched mode only; the one-image loop reads them itself, like the reference), and ship
     their `cam_field` map.  `raw_images`: a step without a network takes the decoded uint8 images themselves (host decode, as
     the reference's VOC12ImageDataset with img_normal=None), whatever --device_pyramid / --device_jpeg say."""
@@ -211,6 +227,10 @@ def make_dataset(args, list_path, scales, cam_dir=None, cam_field="cam", raw_ima
             raise FileNotFoundError("--synthetic_list %s" % names)
         return voc_data.SyntheticMSF(int(args.synthetic), scales=scales, name_list=names, decode_only=decode_only, cam_dir=cam_dir,
                                      cam_field=cam_field)
+    if dataset_name(args) == "coco":
+        from ..coco.dataloader import COCOClassificationDatasetMSF
+        return COCOClassificationDatasetMSF(list_path, coco_root=args.coco_root, cls_labels_path=args.coco_cls_labels, scales=scales,
+                                            decode_only=decode_only, raw_jpeg=device_jpeg(args), cam_dir=cam_dir, cam_field=cam_field)
     return voc_data.VOC12ClassificationDatasetMSF(list_path, voc12_root=args.voc12_root, scales=scales, decode_only=decode_only,
                                                   raw_jpeg=device_jpeg(args), cam_dir=cam_dir, cam_field=cam_field)
 
@@ -483,13 +503,14 @@ def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragge
                   (process_id, ", ".join("%s %.2f" % kv for kv in sorted(ctx.phase_seconds.items(), key=lambda kv: -kv[1]))), file=sys.stderr, flush=True)
 
 
-def run_step(args, work, module_name, class_name, weights_path, strict, list_path, scales, opening="[ ", cam_dir=None, cam_field="cam"):
-    """The reference's `run(args)` (e.g. step/make_cam.py:62-77): model class resolved by name, checkpoint loaded,
-    stride partition (misc/torchutils.py:66-68), one process per GPU (a single GPU runs in-process).  module_name None: a step
-    without a network (step/cam_to_ir_label.py:44-51); `work` then gets model None and the decoded uint8 images."""
+def run_step(args, work, module_name, class_name, weights_path, strict, list_path, scales, opening="[ ", cam_dir=None, cam_field="cam",
+             model_kwargs=None):
+    """The reference's `run(args)` (e.g. step/make_cam.py:62-77): model class resolved by name (constructed with `model_kwargs`),
+    checkpoint loaded, stride partition (misc/torchutils.py:66-68), one process per GPU (a single GPU runs in-process).  module_name
+    None: a step without a network (step/cam_to_ir_label.py:44-51); `work` then gets model None and the decoded uint8 images."""
     model = None
     if module_name is not None:
-        model = getattr(importlib.import_module(module_name), class_name)()
+        model = getattr(importlib.import_module(module_name), class_name)(**(model_kwargs or {}))
         model.load_state_dict(torch.load(weights_path), strict=strict)
         model.eval()
     n_gpus = torch.cuda.device_count()

@@ -22,6 +22,23 @@ def voc_seg_label(voc12_root, img_id):
     return lab
 
 
+def eval_set(args):
+    """(image ids, ground-truth class-index maps with -1 = ignore, n_class) of the evaluation set: VOC's --chainer_eval_set split
+    (21 classes), or with --dataset coco the images of --infer_list, whose ground truth is <--coco_gt_dir>/<name>.png (class index,
+    255 = ignore) over 81 classes."""
+    if str(getattr(args, "dataset", "voc12") or "voc12") != "coco":
+        ids = voc_seg_ids(args.voc12_root, args.chainer_eval_set)
+        return ids, [voc_seg_label(args.voc12_root, i) for i in ids], 21
+    from ..coco import dataloader as coco_data
+    ids = [os.path.basename(s) for s in coco_data.load_stem_list(args.infer_list)]
+    labels = []
+    for i in ids:
+        lab = np.asarray(Image.open(os.path.join(args.coco_gt_dir, i + ".png"))).astype(np.int32)
+        lab[lab == 255] = -1
+        labels.append(lab)
+    return ids, labels, coco_data.N_CAT + 1
+
+
 def confusion(preds, labels, n_class=21):
     """rows = ground truth, cols = prediction; pixels with label < 0 are ignored (step/eval_sem_seg.py:18)."""
     conf = np.zeros((n_class, n_class), np.int64)

@@ -23,7 +23,8 @@ def ir_label_one_image(model, pack, args):
     name = voc_data.decode_int_filename(pack["name"][0])
     cam_dict = np.load(os.path.join(args.cam_out_dir, name + ".npy"), allow_pickle=True).item()
     img = pack["img_u8"].cuda(non_blocking=True)
-    conf = crf.ir_labels(img, [cam_dict["high_res"]], [np.asarray(cam_dict["keys"])], args.conf_fg_thres, args.conf_bg_thres)
+    conf = crf.ir_labels(img, [cam_dict["high_res"]], [np.asarray(cam_dict["keys"])], args.conf_fg_thres, args.conf_bg_thres,
+                         n_classes=_common.n_classes(args))
     _write(conf[0].cpu().numpy(), os.path.join(args.ir_label_out_dir, name + ".png"))
 
 
@@ -44,7 +45,8 @@ def ir_label_batch(ctx, packs):
         flat, sizes = ctx.pack_images(packs)
         x = flat.view((len(packs),) + sizes[0] + (3,))
     with ctx.phase("crf"):
-        conf = crf.ir_labels(x, [torch.as_tensor(h) for h in high], keys, args.conf_fg_thres, args.conf_bg_thres)
+        conf = crf.ir_labels(x, [torch.as_tensor(h) for h in high], keys, args.conf_fg_thres, args.conf_bg_thres,
+                             n_classes=_common.n_classes(args))
     with ctx.phase("hand to writer"):
         ctx.writer.submit(_save, ctx, names, conf, args.ir_label_out_dir)
 

@@ -9,14 +9,13 @@ from . import _voc_eval
 
 
 def run(args):
-    ids = _voc_eval.voc_seg_ids(args.voc12_root, args.chainer_eval_set)
-    labels = [_voc_eval.voc_seg_label(args.voc12_root, i) for i in ids]
+    ids, labels, n_class = _voc_eval.eval_set(args)
     preds = []
     for i in ids:
         p = np.asarray(Image.open(os.path.join(args.sem_seg_out_dir, i + ".png"))).astype(np.uint8).copy()
         p[p == 255] = 0                                                   # step/eval_sem_seg.py:15
         preds.append(p)
-    conf = _voc_eval.confusion(preds, labels)[:21, :21]
+    conf = _voc_eval.confusion(preds, labels, n_class)
     r = _voc_eval.iou_from_confusion(conf)
     print(r["fp"][0], r["fn"][0])
     print(np.mean(r["fp"][1:]), np.mean(r["fn"][1:]))

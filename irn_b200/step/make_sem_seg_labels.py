@@ -58,4 +58,4 @@ def _work(process_id, model, dataset, args):
 
 def run(args):
     _common.run_step(args, _work, args.irn_network, "EdgeDisplacement", args.irn_weights_name, False, args.infer_list, (1.0,), opening="[",
-                     cam_dir=args.cam_out_dir)
+                     cam_dir=args.cam_out_dir, model_kwargs={"crop_size": int(getattr(args, "irn_crop_size", 512))})

@@ -26,10 +26,10 @@ def _fill_trunk(trunk, g):
             m.running_var.data = 1 + 0.2 * torch.rand(c, generator=g)
 
 
-def cam_state_dict(seed=0):
-    """Reference-format state dict for net.resnet50_cam.CAM (956 keys with aliases)."""
+def cam_state_dict(seed=0, n_classes=20):
+    """Reference-format state dict for net.resnet50_cam.CAM (956 keys with aliases), with an `n_classes`-row classifier."""
     g = torch.Generator().manual_seed(seed)
-    m = _params.CamParams()
+    m = _params.CamParams(n_classes)
     _fill_trunk(m.resnet50, g)
     m.classifier.weight.data = 0.01 * torch.randn(m.classifier.weight.shape, generator=g)
     return {k: v.clone() for k, v in m.state_dict().items()}
@@ -79,12 +79,12 @@ def image(index, H=512, W=512):
     return np.clip(np.rint(img), 0, 255).astype(np.uint8)
 
 
-def label(index, n_present=None):
-    """Multi-hot fp32[20] with 1..3 classes (mean ~1.5, like voc12/cls_labels.npy)."""
+def label(index, n_present=None, n_classes=20):
+    """Multi-hot fp32[n_classes] with 1..3 classes (mean ~1.5, like voc12/cls_labels.npy)."""
     rng = np.random.default_rng(977 + int(index))
     k = n_present if n_present is not None else int(rng.choice([1, 2, 3], p=[0.62, 0.30, 0.08]))
-    lab = np.zeros(20, np.float32)
-    lab[rng.choice(20, size=k, replace=False)] = 1
+    lab = np.zeros(n_classes, np.float32)
+    lab[rng.choice(n_classes, size=k, replace=False)] = 1
     return lab
 
 

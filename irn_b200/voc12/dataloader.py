@@ -24,7 +24,10 @@ def cls_labels_dict(path="voc12/cls_labels.npy"):
 
 
 def decode_int_filename(int_filename):
-    """voc12/dataloader.py:26-28 (also accepts the already-decoded 'YYYY_NNNNNN' form)."""
+    """voc12/dataloader.py:26-28 (also accepts the already-decoded 'YYYY_NNNNNN' form; any other name, e.g. an MS COCO file name,
+    is returned as it is)."""
+    if isinstance(int_filename, str) and not int_filename.replace("_", "").isdigit():
+        return int_filename
     s = str(int(str(int_filename).replace("_", "")))
     return s[:4] + "_" + s[4:]
 
@@ -68,7 +71,8 @@ def multi_scale_flip(img_u8, scales, normalize=TorchvisionNormalize()):
 
 class VOC12ClassificationDatasetMSF(Dataset):
     """voc12/dataloader.py:175-205.  Items: {"name": str, "img": list of [2,3,h,w] (or one array),
-    "size": (H, W), "label": FloatTensor[20]}."""
+    "size": (H, W), "label": FloatTensor[20]}.  What is particular to a dataset is in three methods a subclass for another
+    dataset overrides (coco.dataloader): _load_list (the image list and the class labels), item_name and image_path."""
 
     def __init__(self, img_name_list_path, voc12_root, img_normal=TorchvisionNormalize(), scales=(1.0,),
                  cls_labels_path="voc12/cls_labels.npy", decode_only=False, raw_jpeg=False, cam_dir=None, cam_field="cam"):
@@ -76,21 +80,31 @@ class VOC12ClassificationDatasetMSF(Dataset):
         self.decode_only = decode_only      # hand over the decoded uint8 image; the pyramid is built on the device
         self.raw_jpeg = raw_jpeg            # hand over the FILE BYTES; the exact decoder decodes them on the device (irn_b200.jpeg)
         self.cam_dir = cam_dir              # label steps: the loader worker also reads the image's stored CAM dict (make_cam's .npy)
-        self.img_name_list = load_img_name_list(img_name_list_path)
         self.voc12_root = voc12_root
         self.img_normal = img_normal
         self.scales = scales
+        self.img_name_list, self.label_list = self._load_list(img_name_list_path, cls_labels_path)
+
+    def _load_list(self, list_path, cls_labels_path):
+        names = load_img_name_list(list_path)
         labels = cls_labels_dict(cls_labels_path)
-        self.label_list = np.array([labels[int(n)] for n in self.img_name_list])
+        return names, np.array([labels[int(n)] for n in names])
+
+    def item_name(self, idx):
+        """The item's name: the output files of the steps are named after it."""
+        return decode_int_filename(self.img_name_list[idx])
+
+    def image_path(self, idx):
+        return get_img_path(self.item_name(idx), self.voc12_root)
 
     def __len__(self):
         return len(self.img_name_list)
 
     def __getitem__(self, idx):
-        name_str = decode_int_filename(self.img_name_list[idx])
+        name_str = self.item_name(idx)
         if self.raw_jpeg:
             from .. import jpeg, _lib
-            with open(get_img_path(name_str, self.voc12_root), "rb") as f:
+            with open(self.image_path(idx), "rb") as f:
                 data = np.frombuffer(f.read(), dtype=np.uint8).copy()
             try:
                 h, w = jpeg.inspect(data)[:2]
@@ -99,7 +113,7 @@ class VOC12ClassificationDatasetMSF(Dataset):
             else:
                 return attach_cam({"name": name_str, "size": (h, w), "label": torch.from_numpy(self.label_list[idx]), "jpeg_exact": data},
                                   self.cam_dir, self.cam_field)
-        img = np.asarray(Image.open(get_img_path(name_str, self.voc12_root)).convert("RGB"))
+        img = np.asarray(Image.open(self.image_path(idx)).convert("RGB"))
         out = {"name": name_str, "size": (img.shape[0], img.shape[1]), "label": torch.from_numpy(self.label_list[idx])}
         if self.decode_only:
             out["img_u8"] = np.array(img)            # writable copy: torch's collate wraps it without a warning
@@ -127,8 +141,8 @@ class SyntheticMSF(Dataset):
     sizes[i % len(sizes)] (a list of mixed sizes like VOC's); by default every item is `size`."""
 
     def __init__(self, n_items, size=(512, 512), scales=(1.0,), name_list=None, img_normal=TorchvisionNormalize(), decode_only=False,
-                 cam_dir=None, cam_field="cam", sizes=None):
-        self.cam_dir, self.cam_field = cam_dir, cam_field
+                 cam_dir=None, cam_field="cam", sizes=None, n_classes=N_CAT):
+        self.cam_dir, self.cam_field, self.n_classes = cam_dir, cam_field, n_classes
         self.sizes = None if sizes is None else [tuple(int(v) for v in s) for s in sizes]
         self.decode_only = decode_only       # (no module stored on the instance: shards are pickled for spawn / DataLoader workers)
         self.n, self.size, self.scales, self.img_normal = n_items, size, scales, img_normal
@@ -142,7 +156,7 @@ class SyntheticMSF(Dataset):
         from .. import synth
         size = tuple(self.size) if self.sizes is None else self.sizes[idx % len(self.sizes)]
         img = synth.image(idx, *size)
-        out = {"name": name, "size": size, "label": torch.from_numpy(synth.label(idx))}
+        out = {"name": name, "size": size, "label": torch.from_numpy(synth.label(idx, n_classes=self.n_classes))}
         if self.decode_only:
             out["img_u8"] = np.array(img)
         else:

@@ -13,6 +13,11 @@ Differences: --cam_network / --irn_network default to the irn_b200 modules; flag
 any sizes in make_sem_seg_labels / make_ins_seg_labels, of one size in cam_to_ir_label, of one size in make_cam except for buckets
 flushed before they fill, which take smaller images along; 1 = the reference's loop); --device_jpeg True decodes the JPEG
 files the exact device decoder supports on the GPU, bit-identical to the host decode, so every output file is the same.
+
+MS COCO: --dataset coco reads the images named in the lists (path stems relative to --coco_root, one per line) and their class
+labels from --coco_cls_labels (irn_b200/coco/make_cls_labels.py builds it); the class count comes from the CAM checkpoint (80);
+--irn_crop_size 640 takes COCO's largest images; eval_cam and eval_sem_seg score --infer_list against the class-index PNGs in
+--coco_gt_dir over 81 classes (instance AP is VOC only).
 """
 import argparse
 import os
@@ -29,13 +34,21 @@ def _device_jpeg(v):
     return str(v).lower() == "exact" or _bool(v)
 
 
+def _dataset(v):
+    v = str(v).lower()
+    if v not in ("voc12", "coco"):
+        raise argparse.ArgumentTypeError("--dataset is voc12 or coco, got %r" % v)
+    return v
+
+
 def _scales(v):
     return tuple(float(t) for t in str(v).split(","))
 
 
 # (flag, default, type) in the reference's order: environment, dataset, CAM, relation mining, IRNet, random walk, outputs
 FLAGS = [
-    ("num_workers", os.cpu_count() // 2, int), ("voc12_root", "", str), ("synthetic", 0, int), ("synthetic_list", "", str), ("device_pyramid", True, _bool), ("device_jpeg", False, _device_jpeg),
+    ("num_workers", os.cpu_count() // 2, int), ("dataset", "voc12", _dataset), ("voc12_root", "", str), ("coco_root", "", str),
+    ("coco_cls_labels", "coco/cls_labels.npy", str), ("coco_gt_dir", "", str), ("synthetic", 0, int), ("synthetic_list", "", str), ("device_pyramid", True, _bool), ("device_jpeg", False, _device_jpeg),
     ("step_batch", 32, int),
     ("train_list", "voc12/train_aug.txt", str), ("val_list", "voc12/val.txt", str), ("infer_list", "voc12/train.txt", str),
     ("chainer_eval_set", "train", str),
@@ -65,6 +78,12 @@ def parse(argv=None):
     return p.parse_args(argv)
 
 
+def _has_ground_truth(args, eval_pass):
+    if args.dataset == "coco":       # class-index PNGs only: no instance ground truth
+        return eval_pass != "eval_ins_seg" and os.path.isdir(args.coco_gt_dir)
+    return os.path.isdir(os.path.join(args.voc12_root, "SegmentationClass"))
+
+
 def main(argv=None):
     args = parse(argv)
     for d in ("sess", args.cam_out_dir, args.ir_label_out_dir, args.sem_seg_out_dir, args.ins_seg_out_dir):
@@ -81,7 +100,7 @@ def main(argv=None):
     for name in PASSES:
         if not getattr(args, name + "_pass"):
             continue
-        if name in EVAL_STEPS and not args.synthetic and os.path.isdir(os.path.join(args.voc12_root, "SegmentationClass")):
+        if name in EVAL_STEPS and not args.synthetic and _has_ground_truth(args, name):
             pyutils.Timer("step.%s:" % name)
             importlib.import_module("irn_b200.step." + EVAL_STEPS[name]).run(args)
             continue
