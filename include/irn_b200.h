@@ -379,7 +379,8 @@ int irn_jpeg_exact_last_ms(float* ms4);
  * N3  fully connected CRF and the cam_to_ir_label step.  Replaces misc/imutils.py:156-170 (crf_inference_label: pydensecrf's
  * DenseCRF2D with a Gaussian (sxy) and a bilateral (sxy, srgb) Potts term, mean-field inference on the permutohedral lattice)
  * and the body of step/cam_to_ir_label.py:19-41.  The arithmetic is oracle/crf.py's (float32, fixed evaluation order, no
- * floating-point atomics: bitwise reproducible).  A batch is n images of one size; images uint8 [n,H,W,3] (RGB, HWC).
+ * floating-point atomics: bitwise reproducible).  A batch is n images of one size, images uint8 [n,H,W,3] (RGB, HWC), or, through
+ * the _ragged entry points, n images of any sizes packed back to back.
  *
  * irn_crf_workspace_bytes  device workspace for n images with n_groups CRFs each (1: irn_dense_crf, 2: irn_ir_label) of at most
  *                         max_labels labels (<= irn_crf_max_labels()); 0 for arguments no call accepts.
@@ -403,6 +404,24 @@ int irn_dense_crf(const uint8_t* img, const int32_t* labels, int n, int H, int W
 int irn_ir_label(const uint8_t* img, const float* high_res, const int32_t* keys_host, const int32_t* counts_host, int n, int H,
                  int W, float conf_fg_thres, float conf_bg_thres, uint8_t* out, int32_t* vertex_counts, void* workspace,
                  size_t workspace_bytes, irn_stream_t stream);
+/* Ragged batches: sizes_hw HOST int32 [n][2] = (H_i, W_i); every per-image array is image i's one-size array, the images back to back
+ * in batch order (N_i = H_i*W_i; a batch of one size is laid out as above).  Image i's result is, bit for bit, the one-size entry
+ * point's for that image, whatever its neighbours; a batch of equal sizes runs the same kernels as the one-size call.
+ * irn_crf_ragged_workspace_bytes  as irn_crf_workspace_bytes for those sizes (0 for a size <= 0 or a batch too large for one call).
+ * irn_dense_crf_ragged    img uint8 [sum N_i * 3] (img_bytes must be exactly that), labels int32 [sum N_i] -> labels_out int32
+ *                         [sum N_i], q_out fp32 [n_labels * sum N_i] (image i's [n_labels,H_i,W_i] at n_labels * (N_0+..+N_{i-1})).
+ * irn_ir_label_ragged     img as above, high_res fp32 [sum K_i*N_i] (image i's [K_i,H_i,W_i] planes; high_res_elems must be exactly
+ *                         that), keys_host / counts_host as irn_ir_label -> out uint8 [sum N_i].
+ */
+size_t irn_crf_ragged_workspace_bytes(int n, const int32_t* sizes_hw, int n_groups, int max_labels);
+int irn_dense_crf_ragged(const uint8_t* img, size_t img_bytes, const int32_t* sizes_hw, int n, const int32_t* labels, int n_labels,
+                         int t, double gt_prob, float gauss_sxy, float gauss_compat, float bil_sxy, float bil_srgb, float bil_compat,
+                         int32_t* labels_out, float* q_out, int32_t* vertex_counts, void* workspace, size_t workspace_bytes,
+                         irn_stream_t stream);
+int irn_ir_label_ragged(const uint8_t* img, size_t img_bytes, const int32_t* sizes_hw, int n, const float* high_res,
+                        size_t high_res_elems, const int32_t* keys_host, const int32_t* counts_host, float conf_fg_thres,
+                        float conf_bg_thres, uint8_t* out, int32_t* vertex_counts, void* workspace, size_t workspace_bytes,
+                        irn_stream_t stream);
 int irn_crf_set_timing(int enable);
 int irn_crf_last_ms(float* ms3);
 

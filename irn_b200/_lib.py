@@ -96,6 +96,11 @@ SIGNATURES = {
                               c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "irn_ir_label": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_float, c_void_p, c_void_p,
                              c_void_p, c_size_t, c_void_p]),
+    "irn_crf_ragged_workspace_bytes": (c_size_t, [c_int, c_void_p, c_int, c_int]),
+    "irn_dense_crf_ragged": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_void_p, c_int, c_int, c_double, c_float, c_float, c_float,
+                                     c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "irn_ir_label_ragged": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_void_p, c_size_t, c_void_p, c_void_p, c_float, c_float,
+                                    c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "irn_crf_set_timing": (c_int, [c_int]),
     "irn_crf_last_ms": (c_int, [ctypes.POINTER(c_float)]),
 }

@@ -10,11 +10,11 @@ whenever the loader hands over decoded uint8 images: --device_pyramid, the defau
 Batched mode keeps the reference's observable behaviour: same files, same names, same formats; only the order in which
 files appear changes, and file writes overlap the GPU work of the next batch on a small thread pool.  make_sem_seg_labels and
 make_ins_seg_labels batch images of any sizes (IRNet pads every image to crop_size anyway, and the walk on the padded grid is the
-walk on the image's own grid): a batch is every --step_batch consecutive images.  make_cam and cam_to_ir_label work at each image's
-own size: their images are bucketed by size, a bucket is flushed when it holds --step_batch images, when the pending buckets
-together hold more than PENDING_BOUND x --step_batch images (the largest goes), or at the end (Batcher).  make_cam tops up a bucket
-flushed before it is full with smaller images of other sizes, which its CAM forward runs on the bucket's canvas with the padding
-masked, exactly as at their own size.
+walk on the image's own grid), and so does cam_to_ir_label (the CRF builds each image's lattices at its own size within one ragged
+call): a batch is every --step_batch consecutive images.  make_cam works at each image's own size: its images are bucketed by size,
+a bucket is flushed when it holds --step_batch images, when the pending buckets together hold more than PENDING_BOUND x
+--step_batch images (the largest goes), or at the end (Batcher), and a bucket flushed before it is full is topped up with smaller
+images of other sizes, which its CAM forward runs on the bucket's canvas with the padding masked, exactly as at their own size.
 """
 import contextlib
 import importlib
@@ -117,9 +117,9 @@ def device_jpeg(args):
 
 
 def step_batch(args):
-    """--step_batch N (default 32): images processed together -- of any sizes in make_sem_seg_labels and make_ins_seg_labels, of equal
-    size in cam_to_ir_label, of equal size in make_cam except when a bucket is topped up with smaller images; 1 = the reference's
-    one-image loop."""
+    """--step_batch N (default 32): images processed together -- of any sizes in make_sem_seg_labels, make_ins_seg_labels and
+    cam_to_ir_label, of equal size in make_cam except when a bucket is topped up with smaller images; 1 = the reference's one-image
+    loop."""
     return max(1, int(getattr(args, "step_batch", DEFAULT_STEP_BATCH) or 1))
 
 
@@ -135,9 +135,9 @@ def size_key(pack):
 class Batcher:
     """Groups a step's items into batches for `per_batch(ctx, packs)`.
 
-    ragged (the steps whose network runs every image on the padded crop_size canvas, make_sem_seg_labels and
-    make_ins_seg_labels): one pending list, flushed every `bsz` items whatever their sizes.
-    Otherwise (make_cam, cam_to_ir_label, whose work runs at each image's own size): one bucket per size, flushed when it holds
+    ragged (make_sem_seg_labels and make_ins_seg_labels, whose network runs every image on the padded crop_size canvas, and
+    cam_to_ir_label, whose CRF takes images of any sizes in one call): one pending list, flushed every `bsz` items whatever their sizes.
+    Otherwise (make_cam, whose CAM forward runs at each image's own size): one bucket per size, flushed when it holds
     `bsz` items; when more than PENDING_BOUND * bsz items wait in all buckets together, the largest bucket is flushed early, so a
     list with many sizes holds a bounded number of items (each keeps its loader chunk's shared memory alive).  finish() flushes
     what is left.  Every item goes into exactly one batch.
@@ -449,8 +449,8 @@ class StepContext:
 def work_loop(process_id, model, dataset, args, per_image, per_batch=None, ragged=False, riders=False):
     """One GPU's share: the reference's `_work(process_id, model, dataset, args)` signature and loop order
     (step/make_cam.py:16-59), with the per-image / per-batch body supplied by the step.  model None: a step without a network
-    (cam_to_ir_label), whose items are the decoded images themselves.  ragged: per_batch takes images of any sizes; riders: size
-    buckets topped up with smaller images when flushed early (Batcher)."""
+    (cam_to_ir_label), whose items are the decoded images themselves.  ragged: per_batch takes images of any sizes (the label steps
+    and cam_to_ir_label); riders: size buckets topped up with smaller images when flushed early (Batcher, make_cam)."""
     shard = dataset[process_id]
     n_gpus = max(torch.cuda.device_count(), 1)
     scales = getattr(getattr(shard, "dataset", shard), "scales", (1.0,))

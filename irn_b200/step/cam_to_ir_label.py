@@ -28,31 +28,30 @@ def ir_label_one_image(model, pack, args):
     _write(conf[0].cpu().numpy(), os.path.join(args.ir_label_out_dir, name + ".png"))
 
 
-def _save(ctx, names, conf, out_dir):
+def _save(ctx, names, sizes, conf, out_dir):
     (lab,) = ctx.writer.to_host([conf])
-    lab = lab.numpy()
-    for i, name in enumerate(names):
-        ctx.writer.submit_file(_write, lab[i], os.path.join(out_dir, name + ".png"))
+    for name, m in zip(names, crf.unpack(lab, sizes)):
+        ctx.writer.submit_file(_write, m.numpy(), os.path.join(out_dir, name + ".png"))
 
 
 def ir_label_batch(ctx, packs):
-    """The same body for a bucket of equally-sized images: one batched CRF call for all of them."""
+    """The same body for a batch of images of any sizes: one ragged CRF call for all of them (each image's conf map is the one it
+    gets alone)."""
     args = ctx.args
     names = [voc_data.decode_int_filename(p["name"][0]) for p in packs]
     with ctx.phase("cam dicts"):
         keys, high = _common.load_cam_dicts(ctx, packs, names, args.cam_out_dir, field="high_res")
     with ctx.phase("pack + upload images"):
         flat, sizes = ctx.pack_images(packs)
-        x = flat.view((len(packs),) + sizes[0] + (3,))
     with ctx.phase("crf"):
-        conf = crf.ir_labels(x, [torch.as_tensor(h) for h in high], keys, args.conf_fg_thres, args.conf_bg_thres,
-                             n_classes=_common.n_classes(args))
+        conf = crf.ir_labels_ragged(flat, sizes, [torch.as_tensor(h) for h in high], keys, args.conf_fg_thres, args.conf_bg_thres,
+                                    n_classes=_common.n_classes(args))
     with ctx.phase("hand to writer"):
-        ctx.writer.submit(_save, ctx, names, conf, args.ir_label_out_dir)
+        ctx.writer.submit(_save, ctx, names, sizes, conf, args.ir_label_out_dir)
 
 
 def _work(process_id, infer_dataset, args):
-    _common.work_loop(process_id, None, infer_dataset, args, ir_label_one_image, ir_label_batch)
+    _common.work_loop(process_id, None, infer_dataset, args, ir_label_one_image, ir_label_batch, ragged=True)
 
 
 def _work_spawn(process_id, model, dataset, args):

@@ -10,7 +10,7 @@ in the reference's order; the evaluation passes run when VOC ground truth is pre
 Differences: --cam_network / --irn_network default to the irn_b200 modules; flags the reference declares without a type
 (--beta, --exp_times, --*_bg_thres, --*_pass) are parsed; --synthetic N runs on N seeded synthetic images instead of VOC
 (--synthetic_list names them); --step_batch N images are processed together (of
-any sizes in make_sem_seg_labels / make_ins_seg_labels, of one size in cam_to_ir_label, of one size in make_cam except for buckets
+any sizes in make_sem_seg_labels / make_ins_seg_labels / cam_to_ir_label, of one size in make_cam except for buckets
 flushed before they fill, which take smaller images along; 1 = the reference's loop); --device_jpeg True decodes the JPEG
 files the exact device decoder supports on the GPU, bit-identical to the host decode, so every output file is the same.
 
