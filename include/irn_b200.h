@@ -425,6 +425,37 @@ int irn_ir_label_ragged(const uint8_t* img, size_t img_bytes, const int32_t* siz
 int irn_crf_set_timing(int enable);
 int irn_crf_last_ms(float* ms3);
 
+/* ---- MS COCO mask evaluation (irn_b200/csrc/coco_mask.cu) --------------------------------------------------------------------------
+ * Every mask of an H x W image is a bit plane of irn_coco_plane_words(H, W) = W * ceil(H/32) uint32 words: column-major, bit b of word j
+ * of column x = pixel (32j+b, x), the bits past row H-1 zero.  A call's planes lie back to back.  All sizes and descriptors are HOST
+ * arrays, uploaded once per call into the workspace; every output is an exact integer.  Returns -1 for a bad size.
+ *
+ * irn_coco_rasterize   ground truth -> planes uint32 [plane_words], one plane per annotation (ann_hw HOST int32 [n_ann][2] = H, W).
+ *                      An annotation is the union of its parts (part_ann HOST int32 [n_parts]: the part's annotation), each a polygon
+ *                      or an uncompressed RLE.  edges HOST int32 [n_edges][4] = (part, first vertex, k, j): edge j -> j+1 mod k of the
+ *                      part's polygon of k vertices at vertices[first..first+k) (HOST float64 [n_vertices][2] = x, y as in the JSON),
+ *                      every edge of every polygon listed once; toggles HOST int32 [n_toggles][2] = (part, position in [0, H*W]): an
+ *                      RLE's running count sums.  Polygons follow pycocotools' rleFrPoly (coco_mask.cu states the rule).
+ * irn_coco_pack_masks  masks uint8 [sum M_i*H_i*W_i] (image i's bool [M_i,H_i,W_i] back to back, nonzero = inside), hwm HOST int32
+ *                      [n_img][3] = H, W, M -> planes [sum M_i * plane_words(H_i, W_i)].
+ * irn_coco_overlaps    pred / gt planes of n_img images (hwmg HOST int32 [n_img][4] = H, W, M, G; image i's M_i prediction planes and
+ *                      G_i ground-truth planes back to back) -> inter int32 [sum M_i*G_i] (image i's [M_i][G_i] after the earlier
+ *                      images'), area_pred int32 [sum M_i], area_gt int32 [sum G_i].  M_i = 0 or G_i = 0 is allowed.
+ * The workspace queries return 0 for arguments the calls refuse.
+ */
+long long irn_coco_plane_words(int H, int W);
+size_t irn_coco_raster_workspace_bytes(int n_parts, const int32_t* part_hw, int n_edges, int n_vertices, int n_toggles);
+int irn_coco_rasterize(int n_ann, const int32_t* ann_hw, int n_parts, const int32_t* part_ann, int n_edges, const int32_t* edges,
+                       int n_vertices, const double* vertices, int n_toggles, const int32_t* toggles, uint32_t* planes, size_t plane_words,
+                       void* workspace, size_t workspace_bytes, irn_stream_t stream);
+size_t irn_coco_pack_workspace_bytes(int n_img);
+int irn_coco_pack_masks(const uint8_t* masks, size_t mask_bytes, int n_img, const int32_t* hwm, uint32_t* planes, size_t plane_words,
+                        void* workspace, size_t workspace_bytes, irn_stream_t stream);
+size_t irn_coco_overlap_workspace_bytes(int n_img, const int32_t* hwmg);
+int irn_coco_overlaps(const uint32_t* pred_planes, size_t pred_words, const uint32_t* gt_planes, size_t gt_words, int n_img,
+                      const int32_t* hwmg, int32_t* inter, int32_t* area_pred, int32_t* area_gt, void* workspace, size_t workspace_bytes,
+                      irn_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

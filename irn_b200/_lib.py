@@ -103,6 +103,15 @@ SIGNATURES = {
                                     c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "irn_crf_set_timing": (c_int, [c_int]),
     "irn_crf_last_ms": (c_int, [ctypes.POINTER(c_float)]),
+    "irn_coco_plane_words": (ctypes.c_longlong, [c_int, c_int]),
+    "irn_coco_raster_workspace_bytes": (c_size_t, [c_int, c_void_p, c_int, c_int, c_int]),
+    "irn_coco_rasterize": (c_int, [c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_size_t,
+                                   c_void_p, c_size_t, c_void_p]),
+    "irn_coco_pack_workspace_bytes": (c_size_t, [c_int]),
+    "irn_coco_pack_masks": (c_int, [c_void_p, c_size_t, c_int, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p]),
+    "irn_coco_overlap_workspace_bytes": (c_size_t, [c_int, c_void_p]),
+    "irn_coco_overlaps": (c_int, [c_void_p, c_size_t, c_void_p, c_size_t, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                  c_void_p]),
 }
 
 

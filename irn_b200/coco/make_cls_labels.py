@@ -20,10 +20,16 @@ import os
 import numpy as np
 
 
+def category_index(instances):
+    """The class index of every category: (category ids in ascending order, {category id: class k}); class k is the k-th id.  Every
+    module that maps COCO categories to classes goes through this."""
+    cat_ids = sorted(int(c["id"]) for c in instances["categories"])
+    return cat_ids, {c: k for k, c in enumerate(cat_ids)}
+
+
 def cls_labels(instances, image_dir):
     """instances: the parsed annotation file -> ({stem: float32[n_categories]}, sorted category ids)."""
-    cat_ids = sorted(int(c["id"]) for c in instances["categories"])
-    index = {c: k for k, c in enumerate(cat_ids)}
+    cat_ids, index = category_index(instances)
     stem = {}
     labels = {}
     for im in instances["images"]:

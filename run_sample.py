@@ -17,7 +17,11 @@ files the exact device decoder supports on the GPU, bit-identical to the host de
 MS COCO: --dataset coco reads the images named in the lists (path stems relative to --coco_root, one per line) and their class
 labels from --coco_cls_labels (irn_b200/coco/make_cls_labels.py builds it); the class count comes from the CAM checkpoint (80);
 --irn_crop_size 640 takes COCO's largest images; eval_cam and eval_sem_seg score --infer_list against the class-index PNGs in
---coco_gt_dir over 81 classes (instance AP is VOC only).
+--coco_gt_dir over 81 classes, and eval_ins_seg scores the instance labels by COCO mask AP against --coco_instances (an
+instances_*.json; the pass runs only when that file exists).
+
+--make_cocoann_pass True (default False: the reference's driver has no such pass) writes the instance labels of --infer_list as one
+COCO annotation file, --cocoann_out (irn_b200/step/make_cocoann.py).
 """
 import argparse
 import os
@@ -48,7 +52,7 @@ def _scales(v):
 # (flag, default, type) in the reference's order: environment, dataset, CAM, relation mining, IRNet, random walk, outputs
 FLAGS = [
     ("num_workers", os.cpu_count() // 2, int), ("dataset", "voc12", _dataset), ("voc12_root", "", str), ("coco_root", "", str),
-    ("coco_cls_labels", "coco/cls_labels.npy", str), ("coco_gt_dir", "", str), ("synthetic", 0, int), ("synthetic_list", "", str), ("device_pyramid", True, _bool), ("device_jpeg", False, _device_jpeg),
+    ("coco_cls_labels", "coco/cls_labels.npy", str), ("coco_gt_dir", "", str), ("coco_instances", "", str), ("synthetic", 0, int), ("synthetic_list", "", str), ("device_pyramid", True, _bool), ("device_jpeg", False, _device_jpeg),
     ("step_batch", 32, int),
     ("train_list", "voc12/train_aug.txt", str), ("val_list", "voc12/val.txt", str), ("infer_list", "voc12/train.txt", str),
     ("chainer_eval_set", "train", str),
@@ -62,8 +66,11 @@ FLAGS = [
     ("log_name", "sample_train_eval", str), ("cam_weights_name", "sess/res50_cam.pth", str),
     ("irn_weights_name", "sess/res50_irn.pth", str), ("cam_out_dir", "result/cam", str), ("ir_label_out_dir", "result/ir_label", str),
     ("sem_seg_out_dir", "result/sem_seg", str), ("ins_seg_out_dir", "result/ins_seg", str),
+    ("cocoann_out", "voc2012_train_custom.json", str),
 ]
-PASSES = ["train_cam", "make_cam", "eval_cam", "cam_to_ir_label", "train_irn", "make_ins_seg", "eval_ins_seg", "make_sem_seg", "eval_sem_seg"]
+PASSES = ["train_cam", "make_cam", "eval_cam", "cam_to_ir_label", "train_irn", "make_ins_seg", "eval_ins_seg", "make_sem_seg", "eval_sem_seg",
+          "make_cocoann"]
+PASS_DEFAULT_OFF = {"make_cocoann"}     # not a pass of the reference's driver
 HOT_STEPS = {"make_cam": "make_cam", "cam_to_ir_label": "cam_to_ir_label", "make_ins_seg": "make_ins_seg_labels",
              "make_sem_seg": "make_sem_seg_labels"}   # pass -> module
 EVAL_STEPS = {"eval_cam": "eval_cam", "eval_sem_seg": "eval_sem_seg", "eval_ins_seg": "eval_ins_seg"}   # host-side evaluators (need VOC ground truth)
@@ -74,13 +81,15 @@ def parse(argv=None):
     for name, default, typ in FLAGS:
         p.add_argument("--" + name, default=default, type=typ)
     for name in PASSES:
-        p.add_argument("--%s_pass" % name, default=True, type=_bool)
+        p.add_argument("--%s_pass" % name, default=name not in PASS_DEFAULT_OFF, type=_bool)
     return p.parse_args(argv)
 
 
 def _has_ground_truth(args, eval_pass):
-    if args.dataset == "coco":       # class-index PNGs only: no instance ground truth
-        return eval_pass != "eval_ins_seg" and os.path.isdir(args.coco_gt_dir)
+    if args.dataset == "coco":       # class-index PNGs in --coco_gt_dir; instances in --coco_instances
+        if eval_pass == "eval_ins_seg":
+            return os.path.isfile(args.coco_instances)
+        return os.path.isdir(args.coco_gt_dir)
     return os.path.isdir(os.path.join(args.voc12_root, "SegmentationClass"))
 
 
@@ -103,6 +112,9 @@ def main(argv=None):
         if name in EVAL_STEPS and not args.synthetic and _has_ground_truth(args, name):
             pyutils.Timer("step.%s:" % name)
             importlib.import_module("irn_b200.step." + EVAL_STEPS[name]).run(args)
+            continue
+        if name == "make_cocoann":
+            importlib.import_module("irn_b200.step.make_cocoann").run(args)
             continue
         if name not in HOT_STEPS:
             print("[irn_b200] step.%s is outside the native hot path: run the reference's own step for it" % name)
