@@ -14,8 +14,20 @@
  *  - device pointers are BORROWED: the caller (PyTorch in this repo) owns every buffer.  The
  *    library allocates nothing on the device except inside plan objects (irn_net_*) which
  *    hold the repacked network weights.
- *  - all device work is enqueued asynchronously on the caller's stream.
- *  - no global mutable state except constant tables uploaded once per process per device.
+ *  - all device work is enqueued asynchronously on the caller's stream, in call order: every
+ *    launch, memset, CUB pass and copy of a call, including the uploads of its host
+ *    descriptors (which are staged before the call returns, so the host arrays may be reused
+ *    at once).  A call reads its device inputs only after the work enqueued before it on that
+ *    stream.  The calls that return host values (the CRF's vertex counts) synchronise that
+ *    stream only.  Workspaces and scratch buffers are the caller's: two calls in flight at once
+ *    need two of them.
+ *  - calls may come from several host threads at once, each on its own stream; the error text,
+ *    launch counts, last-walk flags and timing switches are per thread.  A net plan (irn_net_*)
+ *    or resize plan used by two threads at once is not covered by this promise.
+ *  - no global mutable state except constant tables uploaded once per process per device, and
+ *    the random walk's radius tables: a call at another radius than the resident one waits for
+ *    every call still enqueueing at the old radius and for the whole device, then uploads
+ *    (so a radius switch cannot happen inside CUDA graph capture).
  *  - tensors are dense row-major; "NCHW"/"NHWC" say which.
  */
 #ifndef IRN_B200_H

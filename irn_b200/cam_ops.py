@@ -6,14 +6,16 @@ import torch
 
 from . import _lib
 from ._params import MAX_CLASSES
+from .indexing import stream_key
 
 
 _scratches = {}
 
 
 def _scratch(dev):
-    """2 x K <= 2 x 128 per-class maxima (int-ordered float bits); one persistent buffer per device, reused in stream order."""
-    key = dev.index
+    """2 x K <= 2 x 128 per-class maxima (int-ordered float bits); one persistent buffer per (device, stream), reused in that stream's
+    order (indexing.stream_key)."""
+    key = stream_key(dev)
     if key not in _scratches:
         _scratches[key] = torch.empty(2 * MAX_CLASSES, dtype=torch.int32, device=dev)
     return _scratches[key]

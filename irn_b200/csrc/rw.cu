@@ -11,6 +11,7 @@
 //   inv_s[img][h][wp] fp64   1 / (1 + sum of the 68 incident weights)
 //   y[2][chan][h][wp] fp64   ping-pong walk state
 #include <mutex>
+#include <shared_mutex>
 #include <type_traits>
 
 #include "common.h"
@@ -33,9 +34,20 @@ struct DevTables {
 };
 __constant__ DevTables c_tab;
 
-static std::mutex g_tab_mutex;
-static int g_tab_radius[64] = {0};   // per device: radius currently resident in c_tab
-static int g_tab_ndst[64] = {0};
+// c_tab holds one radius' tables per device.  Every call that launches kernels reading it holds g_tab_mutex from its check of the
+// resident radius until its last such launch is enqueued: shared while the radius is already resident (calls at one radius, from
+// any number of host threads, never wait for each other), exclusive when it uploads another radius.  So no thread can switch the
+// tables between another thread's check and its launches.
+static std::shared_mutex g_tab_mutex;
+constexpr int kMaxTabDevices = 64;
+static int g_tab_radius[kMaxTabDevices] = {0};   // per device: radius currently resident in c_tab
+static int g_tab_ndst[kMaxTabDevices] = {0};
+
+// Held by a caller of lock_tables until it returns: one of the two locks is engaged.
+struct TableLock {
+    std::shared_lock<std::shared_mutex> shared;
+    std::unique_lock<std::shared_mutex> exclusive;
+};
 
 // Internal plane order for radius 5, grouped by |dx| so the step kernel can stream one |dx| class
 // of planes at a time through shared memory:  class c holds dx=+c (dy = 0..maxdy; dy=0 only exists
@@ -54,11 +66,19 @@ static_assert(plane5(1, 0) == 0 && plane5(0, 1) == 4 && plane5(4, 1) == 8 && pla
                   plane5(4, 3) == -1 && plane5(0, 0) == -1 && plane5(0, -1) == -1,
               "radius-5 plane order");
 
-static int upload_tables(int radius, cudaStream_t stream, int* n_dst_out) {
+// Makes `radius` the resident table of the current device and returns with `lock` holding it there (see g_tab_mutex).
+static int lock_tables(int radius, cudaStream_t stream, int* n_dst_out, TableLock* lock) {
     int dev = 0;
     IRN_CUDA(cudaGetDevice(&dev));
-    std::lock_guard<std::mutex> lock(g_tab_mutex);
-    if (dev < 64 && g_tab_radius[dev] == radius) {
+    if (dev < 0 || dev >= kMaxTabDevices) return fail(kUnsupported, "random walk tables: device index %d >= %d", dev, kMaxTabDevices);
+    lock->shared = std::shared_lock<std::shared_mutex>(g_tab_mutex);
+    if (g_tab_radius[dev] == radius) {
+        if (n_dst_out) *n_dst_out = g_tab_ndst[dev];
+        return kOk;
+    }
+    lock->shared.unlock();
+    lock->exclusive = std::unique_lock<std::shared_mutex>(g_tab_mutex);
+    if (g_tab_radius[dev] == radius) {   // another thread uploaded it in between
         if (n_dst_out) *n_dst_out = g_tab_ndst[dev];
         return kOk;
     }
@@ -66,7 +86,7 @@ static int upload_tables(int radius, cudaStream_t stream, int* n_dst_out) {
     if ((int)t.dst.size() > kMaxDst || (int)t.points.size() > kMaxPts)
         return fail(kUnsupported, "radius %d: %zu destinations / %zu path points exceed the device table", radius,
                     t.dst.size(), t.points.size());
-    static DevTables h;   // guarded by g_tab_mutex
+    static DevTables h;   // guarded by the exclusive g_tab_mutex
     h.n_dst = (int)t.dst.size();
     h.radius = radius;
     for (int k = 0; k < h.n_dst; ++k) {
@@ -82,14 +102,13 @@ static int upload_tables(int radius, cudaStream_t stream, int* n_dst_out) {
         h.px[j] = (signed char)t.points[j].second;
     }
     // Kernels launched earlier on ANY stream may still be reading the previous radius' table: a radius change is rare
-    // (the hot path only uses 5), so wait for the whole device before overwriting the symbol.
+    // (the hot path only uses 5), so wait for the whole device before overwriting the symbol.  (This also makes a radius
+    // switch illegal inside CUDA graph capture.)
     IRN_CUDA(cudaDeviceSynchronize());
     IRN_CUDA(cudaMemcpyToSymbolAsync(c_tab, &h, sizeof(h), 0, cudaMemcpyHostToDevice, stream));
     IRN_CUDA(cudaStreamSynchronize(stream));   // `h` is reused; happens once per (device, radius)
-    if (dev < 64) {
-        g_tab_radius[dev] = radius;
-        g_tab_ndst[dev] = h.n_dst;
-    }
+    g_tab_radius[dev] = radius;
+    g_tab_ndst[dev] = h.n_dst;
     if (n_dst_out) *n_dst_out = h.n_dst;
     return kOk;
 }
@@ -855,7 +874,8 @@ static int walk_impl(const float* x, const float* edge, float* out, int n_img, c
     if (rc) return rc;
     if (((uintptr_t)workspace & 255) != 0) return fail(kBadArg, "irn_random_walk: workspace must be 256-byte aligned");
     int n_dst = 0;
-    rc = upload_tables(radius, stream, &n_dst);
+    TableLock tables;   // held until the last launch reading c_tab is enqueued
+    rc = lock_tables(radius, stream, &n_dst, &tables);
     if (rc) return rc;
     RwWorkspace ws = carve(workspace, n_img, h, w, totc, n_dst);
     if (ws.bytes > workspace_bytes) return fail(kWorkspace, "irn_random_walk: workspace %zu < required %zu bytes", workspace_bytes, ws.bytes);
@@ -921,7 +941,8 @@ extern "C" int irn_edge_to_affinity(const float* edge, float* aff, int n_img, in
     launch_counter() = 0;
     if (!edge || !aff || n_img <= 0 || h <= 0 || w <= 0) return fail(kBadArg, "irn_edge_to_affinity: bad argument");
     if (radius < 2 || radius > 10) return fail(kUnsupported, "irn_edge_to_affinity: radius %d outside [2,10]", radius);
-    int rc = upload_tables(radius, stream, nullptr);
+    TableLock tables;
+    int rc = lock_tables(radius, stream, nullptr, &tables);
     if (rc) return rc;
     return launch_affinity<1>(edge, aff, n_img, h, w, w, radius, 1.0, 1, stream);
 }
@@ -936,7 +957,8 @@ extern "C" int irn_to_affinity_forward(const float* edge, float* aff, int32_t* a
     const int ch = h - R, cw = w - 2 * R;
     if (ch <= 0 || cw <= 0) return fail(kBadArg, "irn_to_affinity_forward: grid %dx%d too small for radius %d", h, w, radius);
     if ((size_t)h * w >= (1u << 31)) return fail(kUnsupported, "irn_to_affinity_forward: grid too large");
-    int rc = upload_tables(radius, stream, nullptr);
+    TableLock tables;
+    int rc = lock_tables(radius, stream, nullptr, &tables);
     if (rc) return rc;
     dim3 grid(((cw + kAffTX - 1) / kAffTX) * ((ch + kAffTY - 1) / kAffTY), n_img), block(kAffTX, kAffTY);
     const size_t smem = (size_t)(kAffTY + R) * (kAffTX + 2 * R) * sizeof(float);
@@ -955,7 +977,8 @@ extern "C" int irn_to_affinity_backward(const float* grad_aff, const int32_t* ar
     const int ch = h - R, cw = w - 2 * R;
     if (ch <= 0 || cw <= 0) return fail(kBadArg, "irn_to_affinity_backward: grid %dx%d too small for radius %d", h, w, radius);
     int n_dst = 0;
-    int rc = upload_tables(radius, stream, &n_dst);
+    TableLock tables;
+    int rc = lock_tables(radius, stream, &n_dst, &tables);
     if (rc) return rc;
     const size_t per_img = (size_t)n_dst * ch * cw, total = per_img * n_img;
     IRN_CUDA(cudaMemsetAsync(grad_edge, 0, (size_t)n_img * h * w * sizeof(float), stream));

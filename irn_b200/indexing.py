@@ -50,11 +50,20 @@ class PathIndex:
             o += n
 
 
+def stream_key(device):
+    """Cache key of the work the caller is about to enqueue: (device index, current stream).  Device buffers cached under it are
+    allocated on that stream and used only by work on that stream, so calls on two streams never share bytes, and dropping a
+    buffer hands it back to the caching allocator in that stream's order, behind every call that used it (no record_stream)."""
+    device = torch.device(device)
+    return device.index, torch.cuda.current_stream(device).cuda_stream
+
+
 _workspaces = {}
 
 
 def _workspace(nbytes, device):
-    key = (device.type, device.index)
+    """Scratch of at least `nbytes` for one call on the current stream of `device`, kept for the next call on that stream."""
+    key = stream_key(device)
     ws = _workspaces.get(key)
     if ws is None or ws.numel() < nbytes:
         ws = torch.empty(int(nbytes * 1.25) + 256, dtype=torch.uint8, device=device)
@@ -66,7 +75,8 @@ _scratches = {}
 
 
 def _scratch(device):
-    key = (device.type, device.index)
+    """rw_labels' global-max word, one per (device, stream) (see stream_key)."""
+    key = stream_key(device)
     if key not in _scratches:
         _scratches[key] = torch.empty(256, dtype=torch.uint8, device=device)
     return _scratches[key]

@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .indexing import _workspace, stream_key
 
 MEAN = (0.485, 0.456, 0.406)
 STD = (0.229, 0.224, 0.225)
@@ -90,10 +91,11 @@ def resize_normalize(imgs_u8, out_hw, mean=MEAN, std=STD, want_u8=False, out=Non
         raise _lib.IrnError("resize_normalize: bad output buffer")
     u8 = torch.empty((B, oh, ow, 3), dtype=torch.uint8, device=dev) if want_u8 else None
     need = L.irn_resize_workspace_bytes(plan.handle, B)
-    ws = _ws.get(dev.index)
+    key = stream_key(dev)      # one workspace per (device, stream): calls on two streams never share it
+    ws = _ws.get(key)
     if ws is None or ws.numel() < need:
         ws = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=dev)
-        _ws[dev.index] = ws
+        _ws[key] = ws
     with torch.cuda.device(dev):
         rc = L.irn_resize_forward(plan.handle, _lib.ptr(x), B, _lib.ptr(out), _lib.ptr(u8), _lib.ptr(ws), ws.numel(), _lib.stream_ptr())
     _lib.check(rc, "irn_resize_forward")
@@ -112,7 +114,6 @@ def resize_normalize_ragged(flat_u8, sizes, scale):
     (h_i, w_i) = rescaled_size(H_i, W_i, scale) (itself at scale 1.0) at the top-left corner of rows 2i (as is) and 2i+1 (W-flipped
     within w_i), +0.0 elsewhere; (Hc, Wc) the largest (h_i, w_i).  Each corner equals resize_normalize of that image alone, bit for bit
     (the loader's MEAN / STD normalisation)."""
-    from .indexing import _workspace
     from .irn import _normalize_lut
     _lib.require_cuda(flat_u8)
     sizes = [(int(h), int(w)) for h, w in sizes]
