@@ -102,13 +102,19 @@ def one_hot(a, n=None):
     return (np.arange(n).reshape((n,) + (1,) * a.ndim) == a[None]).astype(bool)
 
 
-def cluster_centroids(centroids, dp, thres=2.5):
-    """-> bool [I,h,w] (step/make_ins_seg_labels.py:58-75)."""
+def cluster_map(centroids, dp, thres=2.5):
+    """cluster_centroids before its one_hot: int32 [h,w] instance ids in compress_range order (for cases with too many
+    instances to hold the one-hot planes)."""
     strength = np.sqrt(dp[1] ** 2 + dp[0] ** 2)
     h, w = strength.shape
     lab = cc_label(strength < thres).reshape(-1)
     cl = lab[centroids[0] * w + centroids[1]].reshape(h, w)
-    return one_hot(compress_range(cl + 1))
+    return compress_range(cl + 1)
+
+
+def cluster_centroids(centroids, dp, thres=2.5):
+    """-> bool [I,h,w] (step/make_ins_seg_labels.py:58-75)."""
+    return one_hot(cluster_map(centroids, dp, thres))
 
 
 def detect_instance(score_map, mask, class_id, max_fragment_size=0):
