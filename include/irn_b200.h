@@ -144,6 +144,38 @@ int irn_rw_labels(const float* rw, int C, int h, int w, int H, int W, float bg_t
                   void* scratch, irn_stream_t stream);
 
 /* ------------------------------------------------------------------------------------
+ * S1b  background-threshold sweep: the confusion matrices of T background thresholds in one
+ * pass over the scores.  At threshold t a pixel is labelled as by step/eval_cam.py:15-17 or
+ * step/make_sem_seg_labels.py:43-49 with t as the background plane (float32 compare, ties ->
+ * lowest index, the first NaN wins), and counted against its ground truth as
+ * calc_semantic_segmentation_confusion does (255 = ignore).
+ *
+ *  irn_threshold_sweep_bytes: size of the accumulator `hist` for T thresholds (1..256) and
+ *    n_class classes (1..129), 0 when out of range.  The caller zeroes it before the first
+ *    accumulate; every accumulate of a run adds to it.
+ *  irn_threshold_sweep_accumulate: one image.  source IRN_SWEEP_PLANES: scores fp32 [C,H,W]
+ *    used as stored (eval_cam's high_res; h == H, w == W); IRN_SWEEP_WALK: the walk fp32
+ *    [C,h,w], x4 bilinear, cropped to (H,W) and divided by its global max as irn_rw_labels
+ *    does (H <= 4h, W <= 4w; scratch >= 16 bytes).  C = 0: background at every threshold.
+ *    keys_host HOST int32 [C+1], entry 0 = 0 (background);  gt uint8 [H,W];  thresholds_host
+ *    HOST fp32 [T], strictly ascending.  Both tables go to the kernel by value: no copy, no
+ *    synchronisation.  A predicted label or a ground truth (other than 255) >= n_class is
+ *    not counted; it is reported by irn_threshold_sweep_finalize.
+ *  irn_threshold_sweep_finalize: conf int64 [T,n_class,n_class] (rows = ground truth,
+ *    columns = prediction) from `hist`.  Synchronises the stream to read the error words, and
+ *    returns -1 without writing conf if an accumulate met a label >= n_class.
+ */
+#define IRN_SWEEP_PLANES 0
+#define IRN_SWEEP_WALK 1
+size_t irn_threshold_sweep_bytes(int T, int n_class);
+int irn_threshold_sweep_accumulate(int source, const float* scores, int C, int h, int w, int H, int W,
+                                   const int32_t* keys_host, const uint8_t* gt,
+                                   const float* thresholds_host, int T, int n_class, void* hist,
+                                   void* scratch, irn_stream_t stream);
+int irn_threshold_sweep_finalize(const void* hist, int T, int n_class, int64_t* conf,
+                                 irn_stream_t stream);
+
+/* ------------------------------------------------------------------------------------
  * C2/C3  ResNet-50 trunk + CAM head;  I1/I2  IRNet edge / displacement heads.
  * Replace net/resnet50.py:17-91, net/resnet50_cam.py:55-70 (CAM.forward) and
  * net/resnet50_irn.py:23-133,216-234 (Net.forward, MeanShift, EdgeDisplacement.forward).

@@ -217,3 +217,73 @@ def rw_labels(rw, keys, size, bg_thres=0.25, want_index=False, want_scores=False
                              _lib.ptr(scores), _lib.ptr(scratch), _lib.stream_ptr())
     _lib.check(rc, "irn_rw_labels")
     return labels, index, scores
+
+
+class ThresholdSweep:
+    """The confusion matrices of many background thresholds in one pass over the scores (include/irn_b200.h, S1b).  Row j of
+    confusion() is `step._voc_eval.confusion` of the label maps at thresholds[j]: eval_cam's padded argmax for add_cam, rw_labels'
+    for add_walk.  The thresholds are rounded to float32 (the type of the background plane), sorted and deduplicated.  Each stream
+    the adds run on accumulates into a histogram of its own (see stream_key); confusion() finalises and adds them up."""
+
+    def __init__(self, thresholds, n_class, device):
+        t = np.asarray(thresholds, dtype=np.float64).reshape(-1).astype(np.float32)
+        if np.isnan(t).any():
+            raise _lib.IrnError("ThresholdSweep: a threshold is NaN")
+        self.thresholds = np.unique(t)
+        self.n_class = int(n_class)
+        self.device = torch.device(device)
+        self._nbytes = _lib.lib().irn_threshold_sweep_bytes(len(self.thresholds), self.n_class)
+        if self._nbytes == 0:
+            raise _lib.IrnError("ThresholdSweep: %d distinct thresholds and %d classes (need 1..256 and 1..129)" %
+                                (len(self.thresholds), self.n_class))
+        self._acc = {}
+
+    def _add(self, source, scores, C, h, w, keys, size, gt):
+        H, W = int(size[0]), int(size[1])
+        _lib.require_cuda(scores, gt)
+        if scores.device != self.device or gt.device != self.device:
+            raise _lib.IrnError("ThresholdSweep: inputs must be on %s" % self.device)
+        if gt.dtype != torch.uint8 or tuple(gt.shape) != (H, W):
+            raise _lib.IrnError("ThresholdSweep: ground truth must be uint8 [%d,%d], got %s %s" % (H, W, gt.dtype, tuple(gt.shape)))
+        kh = np.ascontiguousarray(np.pad(np.asarray(keys, dtype=np.int64).reshape(-1) + 1, (1, 0)).astype(np.int32))
+        if len(kh) != C + 1:
+            raise _lib.IrnError("ThresholdSweep: %d keys for %d score planes" % (len(kh) - 1, C))
+        key = stream_key(self.device)
+        if key not in self._acc:
+            self._acc[key] = (torch.cuda.current_stream(self.device), torch.zeros(self._nbytes, dtype=torch.uint8, device=self.device),
+                              torch.empty(256, dtype=torch.uint8, device=self.device))
+        _, hist, scratch = self._acc[key]
+        g = gt.contiguous()
+        with torch.cuda.device(self.device):
+            rc = _lib.lib().irn_threshold_sweep_accumulate(source, _lib.ptr(scores), C, h, w, H, W, kh.ctypes.data, _lib.ptr(g),
+                                                           self.thresholds.ctypes.data, len(self.thresholds), self.n_class, _lib.ptr(hist),
+                                                           _lib.ptr(scratch), _lib.stream_ptr())
+        _lib.check(rc, "irn_threshold_sweep_accumulate")
+
+    def add_cam(self, high_res, keys, gt):
+        """high_res cuda fp32 [K,H,W] (make_cam's full-resolution CAMs, K may be 0); keys: the K 0-based class ids; gt cuda uint8 [H,W]
+        (255 = ignore)."""
+        s = high_res.contiguous().float()
+        if s.dim() != 3:
+            raise _lib.IrnError("ThresholdSweep.add_cam: high_res must be [K,H,W], got %s" % (tuple(s.shape),))
+        C, H, W = s.shape
+        self._add(0, s, C, H, W, keys, (H, W), gt)
+
+    def add_walk(self, rw, keys, size, gt):
+        """rw cuda fp32 [C,1,h,w] or [C,h,w] (one image's walk, C may be 0); keys: the C 0-based class ids; size = (H,W); gt cuda uint8
+        [H,W] (255 = ignore)."""
+        h, w = rw.shape[-2:]
+        r = rw.reshape(-1, h, w).contiguous().float()
+        self._add(1, r, r.shape[0], h, w, keys, size, gt)
+
+    def confusion(self):
+        """int64 [T,n_class,n_class] over every image added so far: rows = ground truth, columns = prediction."""
+        T, n = len(self.thresholds), self.n_class
+        out = np.zeros((T, n, n), np.int64)
+        for stream, hist, _ in self._acc.values():
+            with torch.cuda.device(self.device), torch.cuda.stream(stream):
+                conf = torch.empty((T, n, n), dtype=torch.int64, device=self.device)
+                _lib.check(_lib.lib().irn_threshold_sweep_finalize(_lib.ptr(hist), T, n, _lib.ptr(conf), _lib.stream_ptr()),
+                           "irn_threshold_sweep_finalize")
+                out += conf.cpu().numpy()
+        return out

@@ -22,21 +22,32 @@ def voc_seg_label(voc12_root, img_id):
     return lab
 
 
-def eval_set(args):
-    """(image ids, ground-truth class-index maps with -1 = ignore, n_class) of the evaluation set: VOC's --chainer_eval_set split
-    (21 classes), or with --dataset coco the images of --infer_list, whose ground truth is <--coco_gt_dir>/<name>.png (class index,
-    255 = ignore) over 81 classes."""
+def eval_ids(args):
+    """(image ids, n_class) of the evaluation set: VOC's --chainer_eval_set split (21 classes), or with --dataset coco the images of
+    --infer_list over 81 classes."""
     if str(getattr(args, "dataset", "voc12") or "voc12") != "coco":
-        ids = voc_seg_ids(args.voc12_root, args.chainer_eval_set)
-        return ids, [voc_seg_label(args.voc12_root, i) for i in ids], 21
+        return voc_seg_ids(args.voc12_root, args.chainer_eval_set), 21
     from ..coco import dataloader as coco_data
-    ids = [os.path.basename(s) for s in coco_data.load_stem_list(args.infer_list)]
+    return [os.path.basename(s) for s in coco_data.load_stem_list(args.infer_list)], coco_data.N_CAT + 1
+
+
+def gt_png(args, img_id):
+    """The ground-truth PNG of one evaluation image as stored: uint8 class indices, 255 = ignore (VOC's SegmentationClass, or
+    <--coco_gt_dir>/<name>.png with --dataset coco)."""
+    if str(getattr(args, "dataset", "voc12") or "voc12") != "coco":
+        return np.asarray(Image.open(os.path.join(args.voc12_root, "SegmentationClass", img_id + ".png")))
+    return np.asarray(Image.open(os.path.join(args.coco_gt_dir, img_id + ".png")))
+
+
+def eval_set(args):
+    """(image ids, ground-truth class-index maps with -1 = ignore, n_class) of the evaluation set (eval_ids, gt_png)."""
+    ids, n_class = eval_ids(args)
     labels = []
     for i in ids:
-        lab = np.asarray(Image.open(os.path.join(args.coco_gt_dir, i + ".png"))).astype(np.int32)
+        lab = gt_png(args, i).astype(np.int32)
         lab[lab == 255] = -1
         labels.append(lab)
-    return ids, labels, coco_data.N_CAT + 1
+    return ids, labels, n_class
 
 
 def confusion(preds, labels, n_class=21):
@@ -58,6 +69,50 @@ def iou_from_confusion(conf):
     with np.errstate(divide="ignore", invalid="ignore"):
         denom = gtj + resj - diag
         return {"iou": diag / denom, "fp": 1.0 - gtj / denom, "fn": 1.0 - resj / denom}
+
+
+DEFAULT_SWEEP = "0.05:0.95:0.01"     # the threshold sweeps' default candidates (parse_thresholds)
+
+
+def parse_thresholds(v):
+    """A threshold sweep's candidates: a comma list ("0.1,0.15,0.2") or lo:hi:step, expanded as round(lo + i*step, 10) for
+    i = 0 .. floor((hi - lo)/step + 1e-9); a sequence of numbers is taken as it is.  Raises ValueError on anything else."""
+    if not isinstance(v, str):
+        out = [float(t) for t in v]
+    elif ":" in v:
+        parts = v.split(":")
+        if len(parts) != 3:
+            raise ValueError("threshold range %r is not lo:hi:step" % v)
+        lo, hi, step = (float(p) for p in parts)
+        if not (step > 0 and hi >= lo):
+            raise ValueError("threshold range %r needs step > 0 and hi >= lo" % v)
+        out = [round(lo + i * step, 10) for i in range(int(np.floor((hi - lo) / step + 1e-9)) + 1)]
+    else:
+        out = [float(t) for t in v.split(",")]
+    if not out or any(t != t for t in out):
+        raise ValueError("no usable thresholds in %r" % (v,))
+    return out
+
+
+def sweep_scores(thresholds, confs, sem_seg=False):
+    """What eval_cam (sem_seg False) or eval_sem_seg (True) reports at each threshold of a sweep, from its confusion matrices
+    [T,n,n]: one printed line per threshold, then the best one.  Returns {"thresholds": float32 [T], "iou": float64 [T,n],
+    "miou": float64 [T], "best": the threshold of the highest mIoU (the lowest such)}."""
+    ious, mious = [], []
+    for t, conf in zip(thresholds, confs):
+        r = iou_from_confusion(conf)
+        ious.append(r["iou"])
+        mious.append(np.nanmean(r["iou"]))
+        if sem_seg:
+            print("threshold %.6g: miou %.6f  background fp %.6f fn %.6f  mean fp %.6f fn %.6f" %
+                  (t, mious[-1], r["fp"][0], r["fn"][0], np.mean(r["fp"][1:]), np.mean(r["fn"][1:])))
+        else:
+            print("threshold %.6g: miou %.6f" % (t, mious[-1]))
+    mious = np.asarray(mious, np.float64)
+    best = float(thresholds[int(np.nanargmax(mious))]) if np.isfinite(mious).any() else float("nan")
+    print("best threshold %.6g (miou %.6f)" % (best, np.nanmax(mious) if np.isfinite(mious).any() else float("nan")))
+    return {"thresholds": np.asarray(thresholds, np.float32), "iou": np.asarray(ious, np.float64).reshape(len(mious), -1),
+            "miou": mious, "best": best}
 
 
 # ----------------------------------------------------------------------------- instance segmentation (step/eval_ins_seg.py)

@@ -10,12 +10,18 @@ from ..voc12 import dataloader as voc_data
 from . import _common
 
 
-def sem_seg_one_image(model, pack, args):
+def walk_one_image(model, pack, args):
+    """step/make_sem_seg_labels.py:28-41 for one image: (name, class keys, walk [C,1,h,w])."""
     name = voc_data.decode_int_filename(pack["name"][0])
     edge, _ = model(pack["img"][0].cuda(non_blocking=True))
     stored = np.load(os.path.join(args.cam_out_dir, name + ".npy"), allow_pickle=True).item()
     walk = indexing.propagate_to_edge(stored["cam"].cuda(), edge, beta=float(args.beta), exp_times=int(args.exp_times), radius=5)
-    labels, _, _ = indexing.rw_labels(walk, np.asarray(stored["keys"]), pack["size"], float(args.sem_seg_bg_thres))
+    return name, np.asarray(stored["keys"]), walk
+
+
+def sem_seg_one_image(model, pack, args):
+    name, keys, walk = walk_one_image(model, pack, args)
+    labels, _, _ = indexing.rw_labels(walk, keys, pack["size"], float(args.sem_seg_bg_thres))
     Image.fromarray(labels.cpu().numpy()).save(os.path.join(args.sem_seg_out_dir, name + ".png"))
 
 
@@ -31,9 +37,10 @@ def _save(ctx, names, labels, sizes, out_dir):
         o += h * w
 
 
-def sem_seg_batch(ctx, packs):
-    """step/make_sem_seg_labels.py:28-51 for a batch of images of any sizes: one IRNet forward on the padded crop_size canvas, one
-    batched walk on the padded feature grids, each image's walk cropped back to its own grid for the label map."""
+def walk_batch(ctx, packs):
+    """step/make_sem_seg_labels.py:28-41 for a batch of images of any sizes: one IRNet forward on the padded crop_size canvas, one
+    batched walk on the padded feature grids, each image's walk cropped back to its own grid.  Returns (names, keys, walks
+    [C_i,fh_i,fw_i], sizes (H_i,W_i))."""
     args = ctx.args
     names = [voc_data.decode_int_filename(p["name"][0]) for p in packs]
     with ctx.phase("cam dicts"):
@@ -46,6 +53,13 @@ def sem_seg_batch(ctx, packs):
         seeds = _common.to_device_list(ctx, cams)
     with ctx.phase("walk (issue)"):
         rws = ctx.pipe.walk_padded_stage(seeds, edges, sizes)
+    return names, keys, rws, sizes
+
+
+def sem_seg_batch(ctx, packs):
+    """step/make_sem_seg_labels.py:28-51 for a batch of images of any sizes: walk_batch, then each image's label map."""
+    args = ctx.args
+    names, keys, rws, sizes = walk_batch(ctx, packs)
     with ctx.phase("labels (issue)"):
         labels = ctx.pipe.label_ragged_stage(rws, keys, sizes, float(args.sem_seg_bg_thres))
     with ctx.phase("hand to writer"):

@@ -20,6 +20,11 @@ labels from --coco_cls_labels (irn_b200/coco/make_cls_labels.py builds it); the 
 --coco_gt_dir over 81 classes, and eval_ins_seg scores the instance labels by COCO mask AP against --coco_instances (an
 instances_*.json; the pass runs only when that file exists).
 
+Threshold sweeps: --sweep_cam_pass True (after eval_cam) scores the CAMs at every background level of --cam_eval_thres_sweep,
+--sweep_sem_seg_pass True (after eval_sem_seg) the semantic labels at every --sem_seg_bg_thres_sweep (one IRNet forward and one walk
+per evaluation image for all of them); each prints one mIoU line per threshold and the best one.  Both flags take a comma list or
+lo:hi:step (default 0.05:0.95:0.01); both passes are off by default and, like the evaluators, run only where ground truth is present.
+
 --make_cocoann_pass True (default False: the reference's driver has no such pass) writes the instance labels of --infer_list as one
 COCO annotation file, --cocoann_out (irn_b200/step/make_cocoann.py).
 """
@@ -27,6 +32,7 @@ import argparse
 import os
 
 from irn_b200.misc import pyutils
+from irn_b200.step import _voc_eval
 
 
 def _bool(v):
@@ -49,6 +55,14 @@ def _scales(v):
     return tuple(float(t) for t in str(v).split(","))
 
 
+def _thresholds(v):
+    """A threshold sweep's candidates: a comma list, or lo:hi:step (irn_b200.step._voc_eval.parse_thresholds)."""
+    try:
+        return tuple(_voc_eval.parse_thresholds(str(v)))
+    except ValueError as e:
+        raise argparse.ArgumentTypeError(str(e))
+
+
 # (flag, default, type) in the reference's order: environment, dataset, CAM, relation mining, IRNet, random walk, outputs
 FLAGS = [
     ("num_workers", os.cpu_count() // 2, int), ("dataset", "voc12", _dataset), ("voc12_root", "", str), ("coco_root", "", str),
@@ -58,22 +72,26 @@ FLAGS = [
     ("chainer_eval_set", "train", str),
     ("cam_network", "irn_b200.cam", str), ("cam_crop_size", 512, int), ("cam_batch_size", 16, int), ("cam_num_epoches", 5, int),
     ("cam_learning_rate", 0.1, float), ("cam_weight_decay", 1e-4, float), ("cam_eval_thres", 0.15, float),
+    ("cam_eval_thres_sweep", _voc_eval.DEFAULT_SWEEP, _thresholds),
     ("cam_scales", (1.0, 0.5, 1.5, 2.0), _scales),
     ("conf_fg_thres", 0.30, float), ("conf_bg_thres", 0.05, float),
     ("irn_network", "irn_b200.irn", str), ("irn_crop_size", 512, int), ("irn_batch_size", 32, int), ("irn_num_epoches", 3, int),
     ("irn_learning_rate", 0.1, float), ("irn_weight_decay", 1e-4, float),
     ("beta", 10, float), ("exp_times", 8, int), ("ins_seg_bg_thres", 0.25, float), ("sem_seg_bg_thres", 0.25, float),
+    ("sem_seg_bg_thres_sweep", _voc_eval.DEFAULT_SWEEP, _thresholds),
     ("log_name", "sample_train_eval", str), ("cam_weights_name", "sess/res50_cam.pth", str),
     ("irn_weights_name", "sess/res50_irn.pth", str), ("cam_out_dir", "result/cam", str), ("ir_label_out_dir", "result/ir_label", str),
     ("sem_seg_out_dir", "result/sem_seg", str), ("ins_seg_out_dir", "result/ins_seg", str),
     ("cocoann_out", "voc2012_train_custom.json", str),
 ]
-PASSES = ["train_cam", "make_cam", "eval_cam", "cam_to_ir_label", "train_irn", "make_ins_seg", "eval_ins_seg", "make_sem_seg", "eval_sem_seg",
-          "make_cocoann"]
-PASS_DEFAULT_OFF = {"make_cocoann"}     # not a pass of the reference's driver
+PASSES = ["train_cam", "make_cam", "eval_cam", "sweep_cam", "cam_to_ir_label", "train_irn", "make_ins_seg", "eval_ins_seg", "make_sem_seg",
+          "eval_sem_seg", "sweep_sem_seg", "make_cocoann"]
+PASS_DEFAULT_OFF = {"sweep_cam", "sweep_sem_seg", "make_cocoann"}     # not passes of the reference's driver
 HOT_STEPS = {"make_cam": "make_cam", "cam_to_ir_label": "cam_to_ir_label", "make_ins_seg": "make_ins_seg_labels",
              "make_sem_seg": "make_sem_seg_labels"}   # pass -> module
-EVAL_STEPS = {"eval_cam": "eval_cam", "eval_sem_seg": "eval_sem_seg", "eval_ins_seg": "eval_ins_seg"}   # host-side evaluators (need VOC ground truth)
+# evaluators and threshold sweeps: they run only where ground truth is present
+EVAL_STEPS = {"eval_cam": "eval_cam", "eval_sem_seg": "eval_sem_seg", "eval_ins_seg": "eval_ins_seg", "sweep_cam": "sweep_cam",
+              "sweep_sem_seg": "sweep_sem_seg"}
 
 
 def parse(argv=None):
